@@ -73,8 +73,8 @@ struct PathState {
     float4 *hit;       // t, u, v, bits(leaf-order triangle index | kMiss)
     float4 *thr_rng;   // path_throughput.xyz, bits(rng state)
     float4 *radiance;  // per-sample illum.xyz
-    float4 *nee_T;     // throughput before this bounce's update, bits(flags: 4 = missed (environment term pending), 2 = hit (NEE valid), 1 = has shadow ray B)
-    float4 *nee_l1;    // light-sample contribution (without throughput)
+    float4 *nee_T;     // throughput before this bounce's update, bits(flags: 4 = missed (environment term pending), 2 = hit (NEE valid), 1 = has shadow ray B, 8 = has nee_l1)
+    float4 *nee_l1;    // light-sample contribution (without throughput); written only where it passed the pdf tests
     float4 *nee_l2;    // BSDF-sample contribution
     float4 *sray_o;    // shadow ray org.xyz, tfar   (indexed by shadow-queue position)
     float4 *sray_d;    // shadow ray dir.xyz, bits(path slot * 2 + which)
@@ -502,7 +502,12 @@ __global__ void __launch_bounds__(kTravBlock, 8)
 // ---------------------------------------------------------------------------------------
 // 80 registers (6 blocks of 128 per SM) with the three BSDF evaluations inlined measured fastest:
 // 3.19 ms/frame -> 2.67 ms on C2 against 4 blocks x 106 registers with out-of-line BSDF calls
-// (inlining lets the compiler share sub-expressions between disney_pdf and disney_brdf).
+// (inlining lets the compiler share sub-expressions between disney_pdf and disney_brdf; measured on an earlier GPU).
+// With one texture-fetch site for the scalar parameters (unpack_material) the kernel is 7,944 SASS instructions instead
+// of 12,800, and with the shadow rays and NEE terms stored as soon as they are known it spills 4 B instead of 120 B.
+// k_shade's time per C2 frame, all four builds in one run on one H100 SXM (torch.profiler, scripts/profile_frame_launches.py):
+// 3.21 ms before; 2.44 ms at (128, 6) = 80 registers; 2.57 ms at (128, 7) = 72 registers (52 B spilled); 2.85 ms at
+// (128, 8) = 64 registers (140 B spilled). More resident warps do not pay for the spills, so the bounds stay at (128, 6).
 // (A grid-stride form for the thin queues of the late bounces was measured in round 2 and dropped: those launches take
 // ~49 us whatever the grid, and ncu shows why — 12 no-instruction stalls per issued instruction: a warp's first walk
 // through this kernel's ~4000 executed instructions is a chain of instruction-cache misses.)
@@ -516,14 +521,19 @@ __global__ void __launch_bounds__(128, 6) k_shade(DeviceScene sc, PathState ps, 
     uint32_t slot = 0;
     float3 hit_p = mk3(0.f), dir_a = mk3(0.f), dir_b = mk3(0.f);
     float dist_a = 0.f, dist_b = 0.f;
+    // what the continuation needs of a path that hit something
+    bool shaded = false;
+    uint32_t rng = 0u;
+    float3 path_throughput = mk3(0.f), w_o = mk3(0.f), normal = mk3(0.f), v_x = mk3(0.f), v_y = mk3(0.f);
+    DisneyMaterial mat{};
     if (j < count) {
         slot = queue_in[j];
         const float4 ro = ps.ray_o[slot], rd = ps.ray_d[slot], h = ps.hit[slot], tr = ps.thr_rng[slot];
-        float3 path_throughput = mk3(tr.x, tr.y, tr.z);
-        uint32_t rng = __float_as_uint(tr.w);
+        path_throughput = mk3(tr.x, tr.y, tr.z);
+        rng = __float_as_uint(tr.w);
         const uint32_t tri = __float_as_uint(h.w);
         const float3 dir = mk3(rd.x, rd.y, rd.z);
-        const float3 w_o = neg(dir);
+        w_o = neg(dir);
         if (tri == kMiss) {
             // render_embree.ispc:258-262: illum += path_throughput * miss_shader(dir). The environment lookup (atan2f, acosf:
             // ~200 instructions that a warp here would execute for its ~6 missing lanes) is left to k_nee_resolve, which adds
@@ -534,10 +544,11 @@ __global__ void __launch_bounds__(128, 6) k_shade(DeviceScene sc, PathState ps, 
             ps.nee_T[slot] = make_float4(path_throughput.x, path_throughput.y, path_throughput.z, __uint_as_float(4u));
         } else {
             // render_embree.ispc:264-293 (the ray-independent part was precomputed per triangle)
+            shaded = true;
             hit_p = mk3(ro.x + h.x * dir.x, ro.y + h.x * dir.y, ro.z + h.x * dir.z);
             const float4 s0 = __ldg(sc.shade + 3 * (size_t)tri), s1 = __ldg(sc.shade + 3 * (size_t)tri + 1),
                          s2 = __ldg(sc.shade + 3 * (size_t)tri + 2);
-            float3 normal = mk3(s0.x, s0.y, s0.z);
+            normal = mk3(s0.x, s0.y, s0.z);
             const uint32_t material_id = __float_as_uint(s0.w);
             float2 uv = make_float2(0.f, 0.f);
             if (__float_as_uint(s2.z) != 0u) {
@@ -545,23 +556,21 @@ __global__ void __launch_bounds__(128, 6) k_shade(DeviceScene sc, PathState ps, 
                 uv.x = s1.x * bw + s1.z * h.y + s2.x * h.z;
                 uv.y = s1.y * bw + s1.w * h.y + s2.y * h.z;
             }
-            DisneyMaterial mat;
             const TexSource tex_source{sc.texels, sc.tex, sc.tex_objects};
             unpack_material<HWTEX>(mat, sc.materials, material_id, uv, tex_source);
             // render_embree.ispc:296-300
-            float3 v_x, v_y;
             if (mat.specular_transmission == 0.f && dot(w_o, normal) < 0.f) {
                 normal = neg(normal);
             }
             ortho_basis(v_x, v_y, normal);
 
             // ---- sample_direct_light, render_embree.ispc:105-181 ----
-            float3 l1 = mk3(0.f), l2 = mk3(0.f);
+            bool has_l1 = false;
             {
                 uint32_t light_id = (uint32_t)(lcg_randomf(rng) * (float)sc.num_lights);
                 light_id = min(light_id, sc.num_lights - 1u);
-                const QuadLight light = load_light(sc.lights, light_id);
                 {
+                    const QuadLight light = load_light(sc.lights, light_id);
                     const float sx = lcg_randomf(rng);
                     const float sy = lcg_randomf(rng);
                     const float3 light_pos = sample_quad_light_position(light, sx, sy);
@@ -577,13 +586,17 @@ __global__ void __launch_bounds__(128, 6) k_shade(DeviceScene sc, PathState ps, 
                     if (light_pdf >= kEpsilon && bsdf_pdf >= kEpsilon) {
                         const float3 bsdf = disney_brdf(mat, normal, w_o, light_dir, v_x, v_y);
                         const float w = power_heuristic(1.f, light_pdf, 1.f, bsdf_pdf);
-                        l1 = bsdf * light.emission * fabsf(dot(light_dir, normal)) * w / light_pdf;
+                        const float3 l1 = bsdf * light.emission * fabsf(dot(light_dir, normal)) * w / light_pdf;
+                        ps.nee_l1[slot] = make_float4(l1.x, l1.y, l1.z, 0.f);
+                        has_l1 = true;
                     }
                 }
                 {
                     float3 w_i;
                     float bsdf_pdf;
                     const float3 bsdf = sample_disney_brdf(mat, normal, w_o, v_x, v_y, rng, w_i, bsdf_pdf);
+                    // the light again (L1-resident): not live across the sampling
+                    const QuadLight light = load_light(sc.lights, light_id);
                     float light_dist;
                     float3 light_pos;
                     if (!all_zero(bsdf) && bsdf_pdf >= kEpsilon &&
@@ -594,46 +607,20 @@ __global__ void __launch_bounds__(128, 6) k_shade(DeviceScene sc, PathState ps, 
                             emit_b = true;
                             dir_b = w_i;
                             dist_b = light_dist;
-                            l2 = bsdf * light.emission * fabsf(dot(w_i, normal)) * w / bsdf_pdf;
+                            const float3 l2 = bsdf * light.emission * fabsf(dot(w_i, normal)) * w / bsdf_pdf;
+                            ps.nee_l2[slot] = make_float4(l2.x, l2.y, l2.z, 0.f);
                         }
                     }
                 }
             }
+            // bit 1: valid, bit 0: has ray B, bit 3: has a light-sample term. Many light samples fail the pdf tests
+            // (about 42 %, DESIGN.md §2): their shadow ray is still traced and counted, but no zero term is stored or read back.
             ps.nee_T[slot] = make_float4(path_throughput.x, path_throughput.y, path_throughput.z,
-                                         __uint_as_float(emit_b ? 3u : 2u));  // bit 1: valid, bit 0: has ray B
-            ps.nee_l1[slot] = make_float4(l1.x, l1.y, l1.z, 0.f);
-            if (emit_b) {
-                ps.nee_l2[slot] = make_float4(l2.x, l2.y, l2.z, 0.f);
-            }
-
-            // ---- continuation, render_embree.ispc:313-336 ----
-            float pdf;
-            float3 w_i;
-            const float3 bsdf = sample_disney_brdf(mat, normal, w_o, v_x, v_y, rng, w_i, pdf);
-            if (!(pdf == 0.f || all_zero(bsdf))) {
-                path_throughput = path_throughput * bsdf * fabsf(dot(w_i, normal)) / pdf;
-                const int nb = bounce + 1;
-                bool alive = true;
-                if (nb > 3) {
-                    const float q =
-                        fmaxf(0.05f, 1.f - fmaxf(path_throughput.x, fmaxf(path_throughput.y, path_throughput.z)));
-                    if (lcg_randomf(rng) < q) {
-                        alive = false;
-                    } else {
-                        path_throughput = path_throughput / (1.f - q);
-                    }
-                }
-                if (alive && nb < max_depth) {
-                    emit_next = true;
-                    ps.ray_o[slot] = make_float4(hit_p.x, hit_p.y, hit_p.z, kEpsilon);
-                    ps.ray_d[slot] = make_float4(w_i.x, w_i.y, w_i.z, 1e20f);
-                    ps.thr_rng[slot] =
-                        make_float4(path_throughput.x, path_throughput.y, path_throughput.z, __uint_as_float(rng));
-                }
-            }
+                                         __uint_as_float(2u | (emit_b ? 1u : 0u) | (has_l1 ? 8u : 0u)));
         }
     }
-    // ---- compaction: one atomic per warp per queue ----
+    // ---- compaction: one atomic per warp per queue. The shadow rays are stored before the continuation is sampled,
+    // so that their directions and lengths are not live across it (fewer registers; same queues, same image). ----
     const uint32_t ia = warp_append(ps.counters + kCntShadow + bounce, emit_a);
     if (emit_a) {
         ps.sray_o[ia] = make_float4(hit_p.x, hit_p.y, hit_p.z, dist_a);
@@ -643,6 +630,31 @@ __global__ void __launch_bounds__(128, 6) k_shade(DeviceScene sc, PathState ps, 
     if (emit_b) {
         ps.sray_o[ib] = make_float4(hit_p.x, hit_p.y, hit_p.z, dist_b);
         ps.sray_d[ib] = make_float4(dir_b.x, dir_b.y, dir_b.z, __uint_as_float(slot * 2u + 1u));
+    }
+    // ---- continuation, render_embree.ispc:313-336 ----
+    if (shaded) {
+        float pdf;
+        float3 w_i;
+        const float3 bsdf = sample_disney_brdf(mat, normal, w_o, v_x, v_y, rng, w_i, pdf);
+        if (!(pdf == 0.f || all_zero(bsdf))) {
+            path_throughput = path_throughput * bsdf * fabsf(dot(w_i, normal)) / pdf;
+            const int nb = bounce + 1;
+            bool alive = true;
+            if (nb > 3) {
+                const float q = fmaxf(0.05f, 1.f - fmaxf(path_throughput.x, fmaxf(path_throughput.y, path_throughput.z)));
+                if (lcg_randomf(rng) < q) {
+                    alive = false;
+                } else {
+                    path_throughput = path_throughput / (1.f - q);
+                }
+            }
+            if (alive && nb < max_depth) {
+                emit_next = true;
+                ps.ray_o[slot] = make_float4(hit_p.x, hit_p.y, hit_p.z, kEpsilon);
+                ps.ray_d[slot] = make_float4(w_i.x, w_i.y, w_i.z, 1e20f);
+                ps.thr_rng[slot] = make_float4(path_throughput.x, path_throughput.y, path_throughput.z, __uint_as_float(rng));
+            }
+        }
     }
     const uint32_t in = warp_append(ps.counters + kCntQueue + bounce + 1, emit_next);
     if (emit_next) {
@@ -762,7 +774,7 @@ __global__ void __launch_bounds__(256) k_nee_resolve(PathState ps, const uint32_
         continue;
     }
     float3 illum = mk3(0.f);
-    if (ps.vis[2 * slot]) {
+    if ((__float_as_uint(T.w) & 8u) && ps.vis[2 * slot]) {
         const float4 l1 = ps.nee_l1[slot];
         illum = mk3(l1.x, l1.y, l1.z);
     }

@@ -34,6 +34,7 @@ static inline float __uint_as_float(uint32_t u)
     return f;
 }
 static inline float __uint2float_rn(uint32_t u) { return (float)u; }  // x86-64 converts round-to-nearest-even
+static inline int __ffs(unsigned v) { return __builtin_ffs((int)v); }
 using std::max;
 using std::min;
 
@@ -160,6 +161,30 @@ void shadekat_texture(const uint8_t *data, int w, int h, int channels, const flo
         out4n[4 * i + 1] = c.y;
         out4n[4 * i + 2] = c.z;
         out4n[4 * i + 3] = c.w;
+    }
+}
+// the byte -> [0, 1] table texel channels are converted with (kByteToUnit, read through byte_to_unit)
+void shadekat_byte_to_unit(float *out256)
+{
+    for (uint32_t q = 0; q < 256; ++q) {
+        out256[q] = crt::byte_to_unit(q);
+    }
+}
+// unpack_material<false> of material `id` at the n points uv (2n floats) over the RGBA8 arena `texels` and its
+// descriptors `tex` (4 int32 each, DevTex); out: 14 floats per point (base_color.xyz, then the 11 scalar parameters)
+void shadekat_unpack_material(const float *materials, uint32_t id, const uint32_t *texels, const int32_t *tex,
+                              const float *uv, int n, float *out14n)
+{
+    using namespace crt;
+    const TexSource ts{texels, reinterpret_cast<const DevTex *>(tex), nullptr};
+    for (int i = 0; i < n; ++i) {
+        DisneyMaterial m;
+        unpack_material<false>(m, reinterpret_cast<const float4 *>(materials), id, make_float2(uv[2 * i], uv[2 * i + 1]),
+                               ts);
+        const float v[14] = {m.base_color.x, m.base_color.y, m.base_color.z, m.metallic, m.specular, m.roughness,
+                             m.specular_tint, m.anisotropy, m.sheen, m.sheen_tint, m.clearcoat, m.clearcoat_gloss, m.ior,
+                             m.specular_transmission};
+        std::memcpy(out14n + 14 * i, v, sizeof v);
     }
 }
 void shadekat_miss(const float *dirs, int n, float *out3n)

@@ -125,32 +125,59 @@ struct DevTex {
     int32_t width, height;
     int32_t pad;
 };
-CRT_D float4 texel_rgba(const uint32_t *__restrict__ texels, const DevTex t, int x, int y)
+// (float)q / 255.f for every byte q, correctly rounded (the division is done once, by the compiler). A texel channel
+// is converted by a lookup instead of an IEEE division (about ten instructions with its slow-path branch on the
+// device). Global memory read through __ldg, not __constant__: the lanes of a warp look up different bytes, and the
+// constant cache serialises different addresses. tests/test_byte_table_host.py checks every entry bit for bit.
+struct ByteToUnit {
+    float v[256];
+};
+constexpr ByteToUnit make_byte_to_unit()
 {
-    const uint32_t p = __ldg(texels + t.offset + (uint32_t)(y * t.width + x));
-    return make_float4((float)(p & 0xffu) / 255.f, (float)((p >> 8) & 0xffu) / 255.f,
-                       (float)((p >> 16) & 0xffu) / 255.f, (float)(p >> 24) / 255.f);
+    ByteToUnit t{};
+    for (int q = 0; q < 256; ++q) {
+        t.v[q] = (float)q / 255.f;
+    }
+    return t;
 }
-CRT_D float4 texture_rgba(const uint32_t *__restrict__ texels, const DevTex t, const float2 uv)
+__device__ const ByteToUnit kByteToUnit = make_byte_to_unit();
+CRT_D float byte_to_unit(uint32_t q) { return __ldg(kByteToUnit.v + q); }
+
+// The four texel words under the bilinear footprint of uv and the weights of the filter (texture2d.ih:13-83).
+struct TexelQuad {
+    uint32_t p00, p10, p01, p11;
+    float tx, ty;
+};
+CRT_D TexelQuad texel_quad(const uint32_t *__restrict__ texels, const DevTex t, const float2 uv)
 {
     const float ux = uv.x * (float)t.width - 0.5f;
     const float uy = uv.y * (float)t.height - 0.5f;
-    const float tx = ux - floorf(ux);
-    const float ty = uy - floorf(uy);
+    TexelQuad q;
+    q.tx = ux - floorf(ux);
+    q.ty = uy - floorf(uy);
     const int x0 = modi((int)ux, t.width), y0 = modi((int)uy, t.height);
     const int x1 = modi((int)(ux + 1.f), t.width), y1 = modi((int)(uy + 1.f), t.height);
-    const float4 s00 = texel_rgba(texels, t, x0, y0);
-    const float4 s10 = texel_rgba(texels, t, x1, y0);
-    const float4 s01 = texel_rgba(texels, t, x0, y1);
-    const float4 s11 = texel_rgba(texels, t, x1, y1);
-    const float w00 = (1.f - tx), w10 = tx;
-    // s00*(1-tx)*(1-ty) + s10*tx*(1-ty) + s01*(1-tx)*ty + s11*tx*ty, left to right per channel
-    float4 r;
-    r.x = s00.x * w00 * (1.f - ty) + s10.x * w10 * (1.f - ty) + s01.x * w00 * ty + s11.x * w10 * ty;
-    r.y = s00.y * w00 * (1.f - ty) + s10.y * w10 * (1.f - ty) + s01.y * w00 * ty + s11.y * w10 * ty;
-    r.z = s00.z * w00 * (1.f - ty) + s10.z * w10 * (1.f - ty) + s01.z * w00 * ty + s11.z * w10 * ty;
-    r.w = s00.w * w00 * (1.f - ty) + s10.w * w10 * (1.f - ty) + s01.w * w00 * ty + s11.w * w10 * ty;
-    return r;
+    const uint32_t *const base = texels + t.offset;
+    q.p00 = __ldg(base + (uint32_t)(y0 * t.width + x0));
+    q.p10 = __ldg(base + (uint32_t)(y0 * t.width + x1));
+    q.p01 = __ldg(base + (uint32_t)(y1 * t.width + x0));
+    q.p11 = __ldg(base + (uint32_t)(y1 * t.width + x1));
+    return q;
+}
+// One channel (0 = r .. 3 = a) of the filtered texel:
+// s00*(1-tx)*(1-ty) + s10*tx*(1-ty) + s01*(1-tx)*ty + s11*tx*ty, left to right
+CRT_D float bilinear_channel(const TexelQuad &q, uint32_t ch)
+{
+    const uint32_t s = 8u * ch;
+    const float s00 = byte_to_unit((q.p00 >> s) & 0xffu), s10 = byte_to_unit((q.p10 >> s) & 0xffu);
+    const float s01 = byte_to_unit((q.p01 >> s) & 0xffu), s11 = byte_to_unit((q.p11 >> s) & 0xffu);
+    const float w00 = (1.f - q.tx), w10 = q.tx;
+    return s00 * w00 * (1.f - q.ty) + s10 * w10 * (1.f - q.ty) + s01 * w00 * q.ty + s11 * w10 * q.ty;
+}
+CRT_D float4 texture_rgba(const uint32_t *__restrict__ texels, const DevTex t, const float2 uv)
+{
+    const TexelQuad q = texel_quad(texels, t, uv);
+    return make_float4(bilinear_channel(q, 0), bilinear_channel(q, 1), bilinear_channel(q, 2), bilinear_channel(q, 3));
 }
 CRT_D float channel_of(const float4 c, uint32_t ch)
 {
@@ -645,17 +672,7 @@ CRT_D float4 texture_sample(const TexSource &ts, uint32_t tex_id, const float2 u
 #endif
     return texture_rgba(ts.texels, ts.tex[tex_id], uv);
 }
-template <bool HW>
-CRT_D float textured_scalar_param(float x, const float2 uv, const TexSource &ts)
-{
-    const uint32_t mask = __float_as_uint(x);
-    if (mask & 0x80000000u) {
-        const uint32_t tex_id = mask & 0x1fffffffu;
-        const uint32_t channel = (mask >> 29) & 0x3u;
-        return channel_of(texture_sample<HW>(ts, tex_id, uv), channel);
-    }
-    return x;
-}
+// A parameter word with bit 31 set is textured: bits 0-28 the texture id, bits 29-30 the channel of its texel.
 template <bool HW>
 CRT_D void unpack_material(DisneyMaterial &mat, const float4 *__restrict__ materials, uint32_t id, const float2 uv,
                            const TexSource &ts)
@@ -664,22 +681,68 @@ CRT_D void unpack_material(DisneyMaterial &mat, const float4 *__restrict__ mater
                  m2 = __ldg(materials + 4 * id + 2), m3 = __ldg(materials + 4 * id + 3);
     const uint32_t mask = __float_as_uint(m0.x);
     if (mask & 0x80000000u) {
-        const float4 c = texture_sample<HW>(ts, mask & 0x1fffffffu, uv);
-        mat.base_color = mk3(c.x, c.y, c.z);
+        const uint32_t tex_id = mask & 0x1fffffffu;
+        if (HW) {
+            const float4 c = texture_sample<HW>(ts, tex_id, uv);
+            mat.base_color = mk3(c.x, c.y, c.z);
+        } else {
+            const TexelQuad q = texel_quad(ts.texels, ts.tex[tex_id], uv);
+            mat.base_color = mk3(bilinear_channel(q, 0), bilinear_channel(q, 1), bilinear_channel(q, 2));
+        }
     } else {
         mat.base_color = mk3(m0.x, m0.y, m0.z);
     }
-    mat.metallic = textured_scalar_param<HW>(m0.w, uv, ts);
-    mat.specular = textured_scalar_param<HW>(m1.x, uv, ts);
-    mat.roughness = textured_scalar_param<HW>(m1.y, uv, ts);
-    mat.specular_tint = textured_scalar_param<HW>(m1.z, uv, ts);
-    mat.anisotropy = textured_scalar_param<HW>(m1.w, uv, ts);
-    mat.sheen = textured_scalar_param<HW>(m2.x, uv, ts);
-    mat.sheen_tint = textured_scalar_param<HW>(m2.y, uv, ts);
-    mat.clearcoat = textured_scalar_param<HW>(m2.z, uv, ts);
-    mat.clearcoat_gloss = textured_scalar_param<HW>(m2.w, uv, ts);
-    mat.ior = textured_scalar_param<HW>(m3.x, uv, ts);
-    mat.specular_transmission = textured_scalar_param<HW>(m3.y, uv, ts);
+    // The 11 scalar parameters, in the order of their words (m0.w, m1.xyzw, m2.xyzw, m3.xy). The textured ones are
+    // filtered at ONE fetch site, in a loop that is not unrolled: each step filters the one channel it needs, and a
+    // parameter on the same texture as the step before reuses its texel words (the metallic / roughness maps of glTF
+    // share one texture). Inlining a full RGBA fetch per parameter had made this function most of k_shade's code.
+    float p[11] = {m0.w, m1.x, m1.y, m1.z, m1.w, m2.x, m2.y, m2.z, m2.w, m3.x, m3.y};
+    uint32_t textured = 0u;
+#pragma unroll
+    for (int k = 0; k < 11; ++k) {
+        textured |= (__float_as_uint(p[k]) >> 31) << k;
+    }
+    const float *const words = reinterpret_cast<const float *>(materials + 4 * id) + 3;  // words[k] is p[k]
+    uint32_t cur_tex = 0xffffffffu;  // (no texture id: ids have bits 29-31 clear)
+    TexelQuad q{0u, 0u, 0u, 0u, 0.f, 0.f};
+    float4 c = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 1
+    while (textured) {
+        const int k = __ffs(textured) - 1;
+        textured &= textured - 1u;
+        const uint32_t w = __float_as_uint(__ldg(words + k));
+        const uint32_t tex_id = w & 0x1fffffffu, channel = (w >> 29) & 0x3u;
+        float v;
+        if (HW) {
+            if (tex_id != cur_tex) {
+                c = texture_sample<HW>(ts, tex_id, uv);
+            }
+            v = channel_of(c, channel);
+        } else {
+            if (tex_id != cur_tex) {
+                q = texel_quad(ts.texels, ts.tex[tex_id], uv);
+            }
+            v = bilinear_channel(q, channel);
+        }
+        cur_tex = tex_id;
+#pragma unroll
+        for (int j = 0; j < 11; ++j) {  // p[k] = v with k known only at run time: selects keep p in registers
+            if (j == k) {
+                p[j] = v;
+            }
+        }
+    }
+    mat.metallic = p[0];
+    mat.specular = p[1];
+    mat.roughness = p[2];
+    mat.specular_tint = p[3];
+    mat.anisotropy = p[4];
+    mat.sheen = p[5];
+    mat.sheen_tint = p[6];
+    mat.clearcoat = p[7];
+    mat.clearcoat_gloss = p[8];
+    mat.ior = p[9];
+    mat.specular_transmission = p[10];
 }
 // (the software path under its round-1 signature: the test-only host builds call it)
 CRT_D void unpack_material(DisneyMaterial &mat, const float4 *__restrict__ materials, uint32_t id, const float2 uv,
