@@ -110,13 +110,38 @@ CRT_HD float rcp_box(float x)
     return 1.f / x;
 #endif
 }
-CRT_HD float fminf_(float a, float b)
+CRT_HD int32_t imax(int32_t a, int32_t b)
 {
-    return fminf(a, b);
+    return a > b ? a : b;
 }
-CRT_HD float fmaxf_(float a, float b)
+CRT_HD int32_t imin(int32_t a, int32_t b)
 {
-    return fmaxf(a, b);
+    return a < b ? a : b;
+}
+// three-input signed integer max / min: one VIMNMX3 each on sm_90 (DPX)
+CRT_HD int32_t imax3(int32_t a, int32_t b, int32_t c)
+{
+#if defined(__CUDA_ARCH__)
+    return __vimax3_s32(a, b, c);
+#else
+    return imax(a, imax(b, c));
+#endif
+}
+CRT_HD int32_t imin3(int32_t a, int32_t b, int32_t c)
+{
+#if defined(__CUDA_ARCH__)
+    return __vimin3_s32(a, b, c);
+#else
+    return imin(a, imin(b, c));
+#endif
+}
+CRT_HD int32_t f2i(float f)
+{
+    return (int32_t)f2u(f);
+}
+CRT_HD float i2f(int32_t i)
+{
+    return u2f((uint32_t)i);
 }
 
 struct Ray {
@@ -279,6 +304,24 @@ CRT_HD void node_intersect_loaded(const float4 n0, const float4 n1, const float4
     const float obx_lo = obx - sx, obx_hi = obx + sx;
     const float oby_lo = oby - sy, oby_hi = oby + sy;
     const float obz_lo = obz - sz, obz_hi = obz + sz;
+    // Slab test on the float bit patterns as signed integers (Ylitie, Karras and Laine 2017): two three-input integer
+    // min/max and two two-input ones per child instead of six FMNMX, compared as floats.
+    // As signed integers the non-negative floats keep their order and lie above every negative float, and the
+    // negative floats are in reverse order. So over any set of non-NaN values the integer max is at most the float
+    // max (it is equal when the set holds a value >= +0, otherwise it is the most negative element), and the integer
+    // min is at least the float min (equal when every element is >= +0, otherwise it is the negative element closest
+    // to zero). A child the float test accepts is therefore always accepted, whatever the sign of tnear: the test stays
+    // conservative for caller-supplied rays with a negative tnear (crtc_trace_closest). With tnear >= +0, which every
+    // ray of a frame has (k_raygen 0, k_shade and the shadow rays kEpsilon), tmin is exactly the float max, and a
+    // negative tmax rejects the child under both forms (the float compare even keeps tmax = -0.0 against tmin = +0,
+    // as before), so the same children are visited.
+    // NaN would be a large (or, with the sign bit, a small) integer instead of being dropped like fminf / fmaxf do,
+    // so the test relies on no plane distance being NaN. A finite ray (the reciprocals are clamped to |1 / d| <= 1e20)
+    // against a node gives finite ad and ob0 as long as the grid step is below ~3e13 and |p - o| below ~1e18, which
+    // holds for every node the builders emit when the scene and the ray origins lie within +-1e15; after that,
+    // overflow can only reach +-Inf, which orders correctly. A ray with a NaN or Inf component can still make NaN
+    // planes, but tri_test fails for such a ray (NaN-failing comparisons), so it hits nothing either way.
+    const int32_t tnear_i = f2i(ray.tnear), tfar_i = f2i(s.tfar);
     uint32_t hitmask = 0;
 #pragma unroll
     for (int half = 0; half < 2; ++half) {
@@ -301,8 +344,8 @@ CRT_HD void node_intersect_loaded(const float4 n0, const float4 n1, const float4
             const float tmaxx = fma_(byte_unit(xmax, j, s.one), adx, obx_hi);
             const float tmaxy = fma_(byte_unit(ymax, j, s.one), ady, oby_hi);
             const float tmaxz = fma_(byte_unit(zmax, j, s.one), adz, obz_hi);
-            const float tmin = fmaxf_(fmaxf_(tminx, tminy), fmaxf_(tminz, ray.tnear));
-            const float tmax = fminf_(fminf_(tmaxx, tmaxy), fminf_(tmaxz, s.tfar));
+            const float tmin = i2f(imax3(f2i(tminx), f2i(tminy), imax(f2i(tminz), tnear_i)));
+            const float tmax = i2f(imin3(f2i(tmaxx), f2i(tmaxy), imin(f2i(tmaxz), tfar_i)));
             if (tmin <= tmax) {
                 const uint32_t bits = (child_bits4 >> (8 * j)) & 0xffu;
                 const uint32_t idx_ = (bit_index4 >> (8 * j)) & 0xffu;

@@ -156,6 +156,9 @@ __global__ void __launch_bounds__(256) k_raygen(ViewParams view, FrameLayout f, 
 // per lane; the triangles they yield are pooled across the warp and tested 32 pairs at a time
 // (see the loop body). The first kSmemStack entries of each lane's traversal stack live in shared
 // memory, the rest spills to local memory.
+// The 9 launches of a C2 frame take 6.74 ms on an H100 80GB HBM3 at a 400 W power limit (7.02 ms with the FMNMX slab
+// test before the integer one; profiles/launches_c2_h100_traverse_*.md). At (kTravBlock, 8) the kernel has 64 registers
+// and no spills; (128, 9) = 56 registers measured 6.76 ms, (128, 10) = 48 registers spills 42 B and measured 7.89 ms.
 // Profiling hooks of the SIMT emulation (simt_hostcheck.cpp defines them before including this file); they
 // expand to nothing everywhere else, the CUDA build included.
 #ifndef CRT_PROF_NODE_PHASE

@@ -53,8 +53,8 @@ inline void child_boxes(const float4 *nodes, const crt::TravState &s, uint32_t n
             const float tmaxx = fma_(byte_unit(xmax, j, s.one), adx, obx + sx);
             const float tmaxy = fma_(byte_unit(ymax, j, s.one), ady, oby + sy);
             const float tmaxz = fma_(byte_unit(zmax, j, s.one), adz, obz + sz);
-            const float tmin = fmaxf_(fmaxf_(tminx, tminy), fmaxf_(tminz, ray.tnear));
-            const float tmax = fminf_(fminf_(tmaxx, tmaxy), fminf_(tmaxz, s.tfar));
+            const float tmin = fmaxf(fmaxf(tminx, tminy), fmaxf(tminz, ray.tnear));
+            const float tmax = fminf(fminf(tmaxx, tmaxy), fminf(tmaxz, s.tfar));
             tmin8[slot] = tmin;
             hit8[slot] = meta8[slot] != 0 && tmin <= tmax;
             if (tmax8) {

@@ -1,4 +1,4 @@
-"""Per-launch times of one frame of a bench workload, and what the compiler made of k_shade.
+"""Per-launch times of one frame of a bench workload, and what the compiler made of k_shade and k_traverse.
 
     python scripts/profile_frame_launches.py [--workload c2] [--frames 5] [--out FILE.md]
 
@@ -8,9 +8,10 @@ then shade / traversal / NEE resolve per bounce, resolve: 27 launches at depth 8
 its duration over the F frames, followed by the per-kernel sums. The card's name, power limit and maximum SM clock
 are read with nvidia-smi in the same run and written beside the numbers.
 
-Build part (no GPU needed): registers, stack and spill bytes of every k_shade instantiation from the ptxas report
-the Makefile keeps (chameleonrt_b200/csrc/ptxas_info.txt), and their SASS instruction counts from cuobjdump of
-libcrt_cuda_core.so. `--build-only` prints just that part.
+Build part (no GPU needed): registers, stack and spill bytes of every k_shade and k_traverse instantiation from the
+ptxas report the Makefile keeps (chameleonrt_b200/csrc/ptxas_info.txt), and their SASS instruction counts from
+cuobjdump of libcrt_cuda_core.so; for the default k_traverse also where its five node loads sit and the static size of
+its node phase and triangle pass. `--build-only` prints just that part.
 """
 from __future__ import annotations
 
@@ -51,8 +52,20 @@ def ptxas_report(path):
     return out
 
 
-def sass_counts(lib):
-    """{mangled name: SASS instruction count} from cuobjdump -sass, or {} where cuobjdump is not found."""
+TRAVERSE_DEFAULT = "_ZN3crt10k_traverseILb0ELi16ELb0EEEvNS_11DeviceSceneENS_9PathStateEPKjS4_S4_Pjij"
+
+
+def traverse_label(mangled):
+    """k_traverse<COUNT, DEFER, TOP> from its mangled name (the launch options that select each one in parentheses)."""
+    m = re.match(r"_ZN3crt10k_traverseILb(\d)ELi(\d+)ELb(\d)E", mangled)
+    count, defer, top = int(m.group(1)), int(m.group(2)), int(m.group(3))
+    opts = [f"tri_pass_defer {defer}"] + (["count_traversal"] if count else []) + (["bvh_top_smem"] if top else [])
+    default = " (default)" if mangled == TRAVERSE_DEFAULT else ""
+    return f"k_traverse<{'true' if count else 'false'}, {defer}, {'true' if top else 'false'}>{default}: {', '.join(opts)}"
+
+
+def sass_listing(lib):
+    """{mangled name: [(offset, instruction text)]} from cuobjdump -sass, or {} where cuobjdump is not found."""
     exe = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
     if not os.path.exists(exe):
         return {}
@@ -60,18 +73,49 @@ def sass_counts(lib):
     out = {}
     for block in re.split(r"\n\s*Function : ", txt)[1:]:
         name = block.split("\n", 1)[0].strip()
-        out[name] = len(re.findall(r"^\s+/\*[0-9a-f]{4,}\*/\s+\S", block, re.M))
+        out[name] = [(int(o, 16), s.strip()) for o, s in re.findall(r"^\s+/\*([0-9a-f]{4,})\*/\s+([^;]*);", block, re.M)]
     return out
+
+
+def traverse_phases(ins):
+    """Static shape of k_traverse's loop body: the node loads (five 128-bit loads off one base register, offsets
+    0x00..0x40), the node phase from the first of them to the REDUX.SUM that sizes the triangle pass, and the pass from
+    there to its hit merge (the 64-bit shared-memory atomic)."""
+    redux = next((i for i, (_, s) in enumerate(ins) if s.startswith("REDUX.SUM")), None)
+    if redux is None:
+        return None
+    # the last unpredicated 128-bit load of each offset 0x00..0x40 off one base register before the REDUX.SUM
+    last = {}
+    for i, (_, s) in enumerate(ins[:redux]):
+        m = re.match(r"LDG\.E\.128\S* R\d+, desc\[\w+\]\[(R\d+)\.64(?:\+0x([1-4])0)?\]", s)
+        if m:
+            last.setdefault(m.group(1), {})[int(m.group(2) or 0)] = i
+    groups = [sorted(v.values()) for v in last.values() if len(v) == 5]
+    if not groups:
+        return None
+    node = max(groups)
+    merge = next((i for i, (_, s) in enumerate(ins) if i > redux and s.startswith("ATOMS.CAS")), None)
+    return {"node_loads": [ins[j][0] for j in node], "node_phase": redux - node[0],
+            "tri_pass": (merge - redux + 1) if merge is not None else None,
+            "vimnmx3": sum(1 for _, s in ins if s.startswith("VIMNMX3")), "fmnmx": sum(1 for _, s in ins if "FMNMX" in s)}
 
 
 def build_table():
     report = ptxas_report(os.path.join(CSRC, "ptxas_info.txt"))
-    sass = sass_counts(os.path.join(CSRC, "libcrt_cuda_core.so"))
+    sass = sass_listing(os.path.join(CSRC, "libcrt_cuda_core.so"))
     rows = ["| kernel | SASS instructions | registers | stack B | spill stores B | spill loads B |", "|---|---:|---:|---:|---:|---:|"]
-    for mangled, label in SHADE_KERNELS.items():
+    kernels = list(SHADE_KERNELS.items()) + [(m, traverse_label(m)) for m in sorted(report) if m.startswith("_ZN3crt10k_traverse")]
+    for mangled, label in kernels:
         p = report.get(mangled, {})
-        rows.append(f"| `{label}` | {sass.get(mangled, 'n/a')} | {p.get('registers', 'n/a')} | {p.get('stack', 'n/a')} | "
+        n = len(sass[mangled]) if mangled in sass else "n/a"
+        rows.append(f"| `{label}` | {n} | {p.get('registers', 'n/a')} | {p.get('stack', 'n/a')} | "
                     f"{p.get('spill_stores', 'n/a')} | {p.get('spill_loads', 'n/a')} |")
+    ph = traverse_phases(sass[TRAVERSE_DEFAULT]) if TRAVERSE_DEFAULT in sass else None
+    if ph:
+        loads = ", ".join(f"0x{o:04x}" for o in ph["node_loads"])
+        rows += ["", f"Default k_traverse, static: node loads at {loads}; node phase {ph['node_phase']} instructions (first node "
+                     f"load to the pass's REDUX.SUM); triangle pass {ph['tri_pass']} instructions (REDUX.SUM to the 64-bit "
+                     f"shared-memory merge); {ph['vimnmx3']} VIMNMX3, {ph['fmnmx']} FMNMX."]
     return "\n".join(rows)
 
 
@@ -169,7 +213,7 @@ def main():
                   f"GPU (nvidia-smi: name, power limit, max SM clock, driver): {gpu_description()}.", "",
                   f"torch.profiler (CUDA activities), {args.frames} frames after {args.warmup} warm-up frames, one blocking "
                   "render() per frame, stage events off.", "", gpu_table(names, dur, frame_us), ""]
-    parts += ["## k_shade as compiled (ptxas -v, cuobjdump -sass)", "", build_table(), ""]
+    parts += ["## k_shade and k_traverse as compiled (ptxas -v, cuobjdump -sass)", "", build_table(), ""]
     text = "\n".join(parts)
     if args.out:
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
