@@ -72,6 +72,11 @@ RenderCUDA::RenderCUDA(bool native_display_) : native_display(native_display_)
 #endif
     // The plugin API has no option channel (SURVEY.md §5): knobs come from the environment.
     const std::vector<int> devices = devices_from_env();
+    denoise = env_or("CRT_CUDA_DENOISE", 0) != 0;
+    if (denoise && devices.size() > 1) {
+        throw std::runtime_error("crt_cuda: CRT_CUDA_DENOISE needs the whole frame on one GPU; it cannot be combined with "
+                                 "more than one device in CRT_CUDA_DEVICES");
+    }
     try {
         for (size_t i = 0; i < devices.size(); ++i) {
             crtc_renderer *r = nullptr;
@@ -86,6 +91,7 @@ RenderCUDA::RenderCUDA(bool native_display_) : native_display(native_display_)
             check(crtc_set_option(r, "shade_sort", env_or("CRT_CUDA_SHADE_SORT", 0)));  // 1 / 2 = shade queue bucketed by material
             check(crtc_set_option(r, "hw_textures", env_or("CRT_CUDA_HW_TEXTURES", 0)));  // 1 = texels through cudaTextureObject_t (crt_cuda.h)
             check(crtc_set_option(r, "stage_events", env_or("CRT_CUDA_STAGE_EVENTS", 1)));  // 0 = no per-stage timings (crt_cuda_get_stats reads 0)
+            check(crtc_set_option(r, "aov", denoise ? 1 : 0));  // CRT_CUDA_DENOISE: first-hit AOVs for crtc_denoise
         }
     } catch (...) {
         for (crtc_renderer *r : renderers) {
@@ -139,7 +145,8 @@ void RenderCUDA::present_native()
     check_cuda(cudaGraphicsMapResources(1, &cu_display_texture), "cudaGraphicsMapResources");
     cudaArray_t array = nullptr;
     check_cuda(cudaGraphicsSubResourceGetMappedArray(&array, cu_display_texture, 0, 0), "cudaGraphicsSubResourceGetMappedArray");
-    const int rc = crtc_copy_img_to_array(renderers[0], array);  // (every GPU's tiles are in renderers[0]'s frame by then)
+    // (every GPU's tiles are in renderers[0]'s frame by then; CRT_CUDA_DENOISE: the denoised frame instead)
+    const int rc = denoise ? crtc_denoise(renderers[0], nullptr, nullptr, nullptr, array) : crtc_copy_img_to_array(renderers[0], array);
     check_cuda(cudaGraphicsUnmapResources(1, &cu_display_texture), "cudaGraphicsUnmapResources");
     check(rc);
 }
@@ -321,9 +328,12 @@ RenderStats RenderCUDA::render(const glm::vec3 &pos,
                       &up.x,
                       fovy,
                       camera_changed ? 1 : 0,
-                      readback ? 1 : 0,
+                      readback && !denoise ? 1 : 0,
                       img.data(),
                       &s));
+    if (readback && denoise) {
+        check(crtc_denoise(renderer, nullptr, nullptr, img.data(), nullptr));
+    }
 #ifndef CRT_CUDA_HEADLESS
     if (native_display) {
         present_native();

@@ -35,6 +35,9 @@ struct RenderCUDA : RenderCUDABase {
     glm::ivec2 fb_dims = glm::ivec2(0);
     bool native_display = false;
     int frames_since_scene = 0;  // multi-renderer mode: the first frames after set_scene are rendered blocking
+    // CRT_CUDA_DENOISE=1: option "aov" on, and every frame that is read back or presented is the crtc_denoise output
+    // (one renderer only)
+    bool denoise = false;
 
     // native_display: the Display this plugin made is a GLDisplay (render_cuda_plugin.cpp), so frames go to its texture
     // through CUDA-GL interop and `img` is only read back when the application asks (readback_framebuffer: screenshots,

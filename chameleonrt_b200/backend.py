@@ -36,7 +36,17 @@ C_ABI_SYMBOLS = (
     "crtc_initialize", "crtc_set_scene", "crtc_render", "crtc_render_async", "crtc_sync", "crtc_read_accum", "crtc_get_stage_times",
     "crtc_get_counters", "crtc_get_scene_info", "crtc_trace_closest", "crtc_trace_any", "crtc_bench_trace",
     "crtc_local_buffers", "crtc_assemble_rank", "crtc_export_frame", "crtc_import_frame", "crtc_share_frame", "crtc_read_img", "crtc_frame_wait", "crtc_copy_img_to_array",
+    "crtc_read_aov", "crtc_denoise",
 )
+# Per-pixel layout of crtc_read_aov: name -> (first float, number of floats)
+AOV_LAYOUT = {"albedo": (0, 3), "coverage": (3, 1), "normal": (4, 3), "depth": (7, 1), "lum_m1": (8, 1), "lum_m2": (9, 1)}
+AOV_FLOATS = 10
+
+
+class CDenoiseParams(C.Structure):
+    """crtc_denoise_params_t"""
+    _fields_ = [("iterations", C.c_int), ("sigma_luminance", C.c_float), ("sigma_normal", C.c_float),
+                ("sigma_depth", C.c_float)]
 
 
 def lib_path() -> str:
@@ -82,6 +92,8 @@ def load_lib() -> C.CDLL:
     lib.crtc_export_frame.argtypes = [vp, C.c_char_p]
     lib.crtc_import_frame.argtypes = [vp, C.c_char_p]
     lib.crtc_share_frame.argtypes = [vp, vp]
+    lib.crtc_read_aov.argtypes = [vp, vp]
+    lib.crtc_denoise.argtypes = [vp, C.POINTER(CDenoiseParams), vp, vp, vp]
     _lib = lib
     return lib
 
@@ -97,7 +109,7 @@ class RenderCUDA:
     def __init__(self, device: int = 0, max_depth: int = 5, rank: int = 0, world_size: int = 1,
                  count_traversal: bool = False, bvh_threads: int = 0, stream: Optional[int] = None,
                  any_far_first: Optional[int] = None, bvh_builder: Optional[str] = None,
-                 tri_pass_defer: Optional[int] = None, shade_sort: Optional[int] = None):
+                 tri_pass_defer: Optional[int] = None, shade_sort: Optional[int] = None, aov: bool = False):
         self.lib = load_lib()
         self.h = C.c_void_p()
         self._check(self.lib.crtc_create(C.byref(self.h), device))
@@ -133,6 +145,8 @@ class RenderCUDA:
             if bvh_builder not in names:
                 raise ValueError(f"bvh_builder must be one of {names}")
             self._check(self.lib.crtc_set_option(self.h, b"bvh_builder", names.index(bvh_builder)))
+        if aov:  # first-hit AOVs with every frame, for read_aov() and denoise() (crt_cuda.h: option "aov")
+            self._check(self.lib.crtc_set_option(self.h, b"aov", 1))
         if stream is not None:
             self._check(self.lib.crtc_set_stream(self.h, C.c_void_p(stream)))
         self.width = self.height = 0
@@ -232,6 +246,24 @@ class RenderCUDA:
         assert out.dtype == np.uint32 and out.shape == (self.height, self.width) and out.flags["C_CONTIGUOUS"]
         self._check(self.lib.crtc_read_img(self.h, out.ctypes.data))
         return out
+
+    def read_aov(self) -> dict:
+        """The accumulated first-hit AOVs (crtc_read_aov; needs ``aov=True``): ``albedo`` (h, w, 3), ``coverage`` (h, w),
+        ``normal`` (h, w, 3, the mean normal, not renormalised), ``depth`` (h, w), ``lum_m1`` / ``lum_m2`` (h, w: the
+        mean of the sample luminance and of its square), all float32."""
+        a = np.zeros((self.height, self.width, AOV_FLOATS), dtype=np.float32)
+        self._check(self.lib.crtc_read_aov(self.h, a.ctypes.data))
+        return {k: (a[:, :, o:o + n] if n > 1 else a[:, :, o]).copy() for k, (o, n) in AOV_LAYOUT.items()}
+
+    def denoise(self, iterations: int = 5, sigma_luminance: float = 4.0, sigma_normal: float = 128.0,
+                sigma_depth: float = 1.0):
+        """Edge-aware à-trous denoiser over the accumulated frame (crtc_denoise; needs ``aov=True``). Returns
+        (rgb (h, w, 3) float32, img (h, w) uint32 RGBA8)."""
+        prm = CDenoiseParams(int(iterations), float(sigma_luminance), float(sigma_normal), float(sigma_depth))
+        rgb = np.zeros((self.height, self.width, 3), dtype=np.float32)
+        img = np.zeros((self.height, self.width), dtype=np.uint32)
+        self._check(self.lib.crtc_denoise(self.h, C.byref(prm), rgb.ctypes.data, img.ctypes.data, None))
+        return rgb, img
 
     def stage_times(self) -> dict:
         a = np.zeros(len(STAGE_NAMES), dtype=np.float32)

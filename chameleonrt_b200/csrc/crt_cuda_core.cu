@@ -17,6 +17,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/crt_cuda.h"
+#include "aov_denoise.cuh"
 #include "bvh8.h"
 #include "cuda_host_utils.h"
 #include "host_scene.h"
@@ -226,6 +227,27 @@ struct crtc_renderer {
     DeviceBuffer<float> d_accum_local, d_accum_full;
     DeviceBuffer<uint32_t> d_img_local, d_img_full;
 
+    // option "aov" (aov_denoise.cuh): first-hit AOVs accumulated with the frame, and the denoiser over them. `aov` is the
+    // option, `aov_active` what the last crtc_initialize set up.
+    bool aov = false, aov_active = false;
+    crt::AovState aov_state;
+    void require_unshared_aov(const char *what) const
+    {
+        if (aov_active) {
+            throw std::runtime_error(std::string(what) + ": the AOVs and the denoiser need the whole frame on one renderer; "
+                                     "this renderer was initialized with option aov = 1");
+        }
+    }
+    void require_aov_frame(const char *what) const
+    {
+        if (!aov_active) {
+            throw std::runtime_error(std::string(what) + ": option aov is off (set it to 1 before crtc_initialize)");
+        }
+        if (frame_id == 0) {
+            throw std::runtime_error(std::string(what) + ": no frame has been rendered since the last reset");
+        }
+    }
+
     // frames: records of enqueued-but-not-collected frames, and a pool of reusable ones
     std::vector<std::unique_ptr<FrameRecord>> in_flight, record_pool;
     float stage_ms[kNumStages] = {0};   // last collected frame
@@ -306,6 +328,8 @@ struct crtc_renderer {
         if (fb_w == 0 || dst->fb_w != fb_w || dst->fb_h != fb_h) {
             throw std::runtime_error("crtc_share_frame: both renderers must be initialized with the same size");
         }
+        require_unshared_aov("crtc_share_frame");
+        dst->require_unshared_aov("crtc_share_frame");
         make_current();
         close_peer_frame();
         if (dst->device != device) {
@@ -338,6 +362,7 @@ struct crtc_renderer {
         if (fb_w == 0) {
             throw std::runtime_error("crtc_export_frame: initialize() has not been called");
         }
+        require_unshared_aov("crtc_export_frame");
         make_current();
         static_assert(sizeof(cudaIpcMemHandle_t) == 64, "two 64-byte handles");
         cudaIpcMemHandle_t h[2];
@@ -354,6 +379,7 @@ struct crtc_renderer {
         if (!handles) {
             return;
         }
+        require_unshared_aov("crtc_import_frame");
         cudaIpcMemHandle_t h[2];
         std::memcpy(h, handles, sizeof(h));
         void *a = nullptr, *i = nullptr;
@@ -576,6 +602,10 @@ struct crtc_renderer {
         if (w <= 0 || h <= 0) {
             throw std::runtime_error("initialize: framebuffer dimensions must be positive");
         }
+        if (aov && world_size > 1) {
+            throw std::runtime_error("initialize: option aov needs the whole frame on one renderer (world_size 1); "
+                                     "AOVs of multi-GPU frames are not supported");
+        }
         make_current();
         CUDA_CHECK(cudaStreamSynchronize(stream));
         unpin_img();             // (the caller's img buffer is reallocated with the new size)
@@ -606,6 +636,12 @@ struct crtc_renderer {
         }
         CUDA_CHECK(cudaMemsetAsync(d_accum_full.ptr, 0, (size_t)w * h * 3 * sizeof(float), stream));
         CUDA_CHECK(cudaMemsetAsync(d_img_full.ptr, 0, ((size_t)w * h + crt::kSyncWords) * 4, stream));
+        aov_active = aov;
+        if (aov_active) {
+            aov_state.allocate(npx_local, (size_t)w * h, stream);
+        } else {
+            aov_state.release();
+        }
         share_seq = 0;
         CUDA_CHECK(cudaStreamSynchronize(stream));
     }
@@ -739,6 +775,9 @@ struct crtc_renderer {
         scene_info[11] = (bvh_builder == 1 && built_on_device) ? (double)build_rounds : 0.0;
         if (npx_local) {
             CUDA_CHECK(cudaMemsetAsync(d_accum_local.ptr, 0, (size_t)npx_local * 3 * sizeof(float), stream));
+            if (aov_active) {
+                CUDA_CHECK(cudaMemsetAsync(aov_state.local.ptr, 0, (size_t)npx_local * crt::kAovFloats * sizeof(float), stream));
+            }
         }
     }
 
@@ -841,6 +880,10 @@ struct crtc_renderer {
             launch_traverse(sc, ps, ps.queue[0], ps.counters + crt::kCntQueue, nullptr, ps.counters + crt::kCntWork);
             rec.mark(stream, kStPrimary);
             rec.launches += 2;
+            if (aov_active) {  // (its time counts as shading: the next mark closes the stage)
+                aov_state.launch_primary(sc, fl, ps, frame_id, stream);
+                rec.launches += 1;
+            }
             for (int b = 0; b < max_depth; ++b) {
                 const uint32_t *qin = ps.queue[b & 1];
                 uint32_t *qout = ps.queue[(b + 1) & 1];
@@ -886,6 +929,10 @@ struct crtc_renderer {
             crt::k_resolve<<<gpx, 256, 0, stream>>>(fl, ps, frame_id, d_accum_local.ptr, d_img_local.ptr, full_accum, full_img,
                                                    d_done_counter.ptr, arrive, share_seq + 1u);
             rec.launches += 1;
+            if (aov_active) {  // (counted in the resolve stage)
+                aov_state.launch_moments(fl, ps, frame_id, stream);
+                rec.launches += 1;
+            }
             rec.mark(stream, kStResolve);
         } else if (shared_src) {
             // a rank that owns no tile of this frame (more ranks than tiles) still has to say "done"
@@ -1148,6 +1195,52 @@ struct crtc_renderer {
         return ms / iters;
     }
 
+    void read_aov(float *out)
+    {
+        require_aov_frame("crtc_read_aov");
+        make_current();
+        CUDA_CHECK(cudaMemcpyAsync(out, aov_state.full.ptr, (size_t)fb_w * fb_h * crt::kAovFloats * sizeof(float),
+                                   cudaMemcpyDeviceToHost, stream));
+        CUDA_CHECK(cudaStreamSynchronize(stream));
+        CUDA_CHECK(cudaGetLastError());
+    }
+
+    void denoise(const crtc_denoise_params_t *params, float *rgb_out, uint32_t *img_out, void *cuda_array)
+    {
+        crt::DenoiseParams p;
+        if (params) {
+            if (params->iterations < 1 || params->iterations > 10) {
+                throw std::runtime_error("crtc_denoise: iterations must be in [1, 10]");
+            }
+            const float s[3] = {params->sigma_luminance, params->sigma_normal, params->sigma_depth};
+            for (float v : s) {
+                if (!std::isfinite(v) || !(v > 0.f)) {
+                    throw std::runtime_error("crtc_denoise: sigma_luminance, sigma_normal and sigma_depth must be finite and > 0");
+                }
+            }
+            p.iterations = params->iterations;
+            p.sigma_l = s[0];
+            p.sigma_n = s[1];
+            p.sigma_z = s[2];
+        }
+        require_aov_frame("crtc_denoise");
+        make_current();
+        aov_state.denoise(fb_w, fb_h, (float)spp * (float)frame_id, d_accum_full.ptr, p, stream);
+        const size_t n = (size_t)fb_w * fb_h;
+        if (rgb_out) {
+            CUDA_CHECK(cudaMemcpyAsync(rgb_out, aov_state.dn_rgb.ptr, n * 3 * sizeof(float), cudaMemcpyDeviceToHost, stream));
+        }
+        if (img_out) {
+            CUDA_CHECK(cudaMemcpyAsync(img_out, aov_state.dn_img.ptr, n * 4, cudaMemcpyDeviceToHost, stream));
+        }
+        if (cuda_array) {
+            CUDA_CHECK(cudaMemcpy2DToArrayAsync(static_cast<cudaArray_t>(cuda_array), 0, 0, aov_state.dn_img.ptr, (size_t)fb_w * 4,
+                                                (size_t)fb_w * 4, (size_t)fb_h, cudaMemcpyDeviceToDevice, stream));
+        }
+        CUDA_CHECK(cudaStreamSynchronize(stream));
+        CUDA_CHECK(cudaGetLastError());
+    }
+
     // tile-id lists of the other ranks, cached on the device (keyed by world_size * 4096 + rank)
     std::vector<std::pair<int, std::unique_ptr<DeviceBuffer<uint32_t>>>> assemble_tiles;
 
@@ -1310,6 +1403,8 @@ int crtc_set_option(crtc_renderer *r, const char *key, int64_t value)
             r->bvh_builder = (int)value;
         } else if (k == "count_traversal") {
             r->count_traversal = value != 0;
+        } else if (k == "aov") {
+            r->aov = value != 0;  // takes effect at the next crtc_initialize
         } else if (k == "refill_idle") {
             r->refill_idle = (int)std::min<int64_t>(std::max<int64_t>(value, 1), 32);
         } else if (k == "any_far_first") {
@@ -1355,6 +1450,8 @@ int crtc_get_option(crtc_renderer *r, const char *key, int64_t *value)
             *value = r->build_rounds;  // PLOC rounds of the last device build
         } else if (k == "count_traversal") {
             *value = r->count_traversal ? 1 : 0;
+        } else if (k == "aov") {
+            *value = r->aov ? 1 : 0;
         } else if (k == "refill_idle") {
             *value = r->refill_idle;
         } else if (k == "any_far_first") {
@@ -1441,6 +1538,21 @@ int crtc_read_img(crtc_renderer *r, uint32_t *img)
         CUDA_CHECK(cudaStreamSynchronize(r->stream));
         r->check_sync_error();
     })
+}
+
+int crtc_read_aov(crtc_renderer *r, float *out)
+{
+    CRTC_TRY({ require_renderer(r);
+        if (!out) {
+            throw std::runtime_error("crtc_read_aov: out is NULL");
+        }
+        r->read_aov(out);
+    })
+}
+
+int crtc_denoise(crtc_renderer *r, const crtc_denoise_params_t *params, float *rgb_out, uint32_t *img_out, void *cuda_array)
+{
+    CRTC_TRY({ require_renderer(r); r->denoise(params, rgb_out, img_out, cuda_array); })
 }
 
 int crtc_get_stage_times(crtc_renderer *r, float *ms_out, int n)

@@ -101,6 +101,15 @@ void crtc_destroy(crtc_renderer *r);
  *                 stage was at least 3 % faster. 0 = off.
  *   "count_traversal" 1 = instrumented traversal kernels that count node visits and triangle
  *                 tests (for the algorithmic-byte figure; slower, off by default)
+ *   "aov"         0 (default) / 1: first-hit AOV buffers accumulated with every frame, read with crtc_read_aov and used by
+ *                 crtc_denoise. Takes effect at the next crtc_initialize. Needs the whole frame on one renderer: with
+ *                 world_size > 1 crtc_initialize fails, and crtc_export_frame / crtc_import_frame / crtc_share_frame fail
+ *                 on a renderer initialized with it. Two kernels per wavefront (k_aov_primary after the primary traversal,
+ *                 k_aov_moments after the resolve), so counter [2] (kernel launches) grows by 2 per wavefront; their
+ *                 times are counted in stage [2] (shade) and [5] (resolve) of crtc_get_stage_times. They read the path
+ *                 state and write only their own buffers: accum, img and the ray counts are the same with the option on.
+ *                 Memory: 40 B per pixel of the local tiles (64x64-padded) + 40 B per framebuffer pixel; the first
+ *                 crtc_denoise adds 72 B per framebuffer pixel (1920x1080: 166 MB of AOVs + 149 MB for the denoiser).
  */
 int crtc_set_option(crtc_renderer *r, const char *key, int64_t value);
 
@@ -215,6 +224,40 @@ int crtc_copy_img_to_array(crtc_renderer *r, void *cuda_array);
 /* Read the assembled full frame (after crtc_assemble_rank for every rank, after every rank's peer-written
  * frame has completed, or after a world_size==1 render). */
 int crtc_read_img(crtc_renderer *r, uint32_t *img);
+
+/* Option "aov": the accumulated first-hit AOVs, fb_width*fb_height*10 floats, row-major, per pixel: albedo.rgb, coverage,
+ * normal.xyz, depth, lum_m1, lum_m2. Each is a running mean over the frames since the last reset (crtc_initialize,
+ * crtc_set_scene, camera_changed), with crtc_read_accum's formula, of the frame's mean over its spp samples:
+ *   albedo    the base colour of the primary hit as the shading kernel unpacks it; the miss shader's colour on a miss
+ *   coverage  the fraction of samples that hit geometry
+ *   normal    the shading normal of the hit, face-forwarded as the shading kernel does it (0 on a miss); not renormalised
+ *   depth     the hit distance along the primary ray, averaged over the samples that hit (0 if none did)
+ *   lum_m1/2  mean of L and of L^2 over the samples, L = 0.2126 r + 0.7152 g + 0.0722 b of a sample's radiance
+ * Fails if the option is off or no frame has been rendered since the last reset. */
+int crtc_read_aov(crtc_renderer *r, float *out);
+
+typedef struct crtc_denoise_params_t {
+    int iterations;        /* K, 1..10 (default 5): a-trous steps 1, 2, 4, ... 2^(K-1) pixels */
+    float sigma_luminance; /* default 4:   w_l = exp(-|l_p - l_q| / (sigma_luminance * sqrt(blurred variance) + 1e-10)) */
+    float sigma_normal;    /* default 128: w_n = max(0, dot(n_p, n_q))^sigma_normal */
+    float sigma_depth;     /* default 1:   w_z = exp(-|Z_p - Z_q| / (sigma_depth * |grad Z_p . step offset| + 1e-3)) */
+} crtc_denoise_params_t;
+
+/* Edge-aware a-trous denoiser over the accumulated frame (the spatial part of SVGF, Schied et al. 2017; no temporal
+ * reprojection: accumulation covers a still camera). Needs option "aov" and a frame, like crtc_read_aov.
+ *   1. I = accum / max(albedo, 1e-3) per channel; v = max(0, lum_m2 - lum_m1^2) / (spp * frames accumulated).
+ *   2. K iterations i = 0..K-1 with step h = 2^i over a 5x5 B3-spline kernel (1,4,6,4,1)/16 per axis, taps outside the
+ *      image skipped, dy outer and dx inner. Per tap q of pixel p: w = k * w_l * w_n * w_z, where the luminance weight
+ *      uses g_p = the 3x3 (1,2,1)x(1,2,1)/16 blur of v at p (normalised over the taps inside the image), the normal
+ *      weight uses unit normals (1 if both pixels have no normal, 0 if exactly one has none) and the depth weight uses
+ *      the central difference of the depth (one-sided at the borders) dotted with h*(dx, dy).
+ *      I' = sum w I_q / sum w, v' = sum w^2 v_q / (sum w)^2.
+ *   3. rgb = I' * max(albedo, 1e-3), img = its sRGB8 conversion (as the frame's own img), alpha 255.
+ * params: NULL = the defaults; out of range (iterations outside 1..10, a sigma not finite or <= 0) is an error.
+ * Outputs, each optional: rgb_out (HOST, fb_width*fb_height*3 floats), img_out (HOST, fb_width*fb_height RGBA8),
+ * cuda_array (a cudaArray_t, as crtc_copy_img_to_array). All work runs on the renderer's stream (crtc_set_stream); returns
+ * when the outputs are written. Scratch buffers (72 B per pixel) are allocated by the first call after crtc_initialize. */
+int crtc_denoise(crtc_renderer *r, const crtc_denoise_params_t *params, float *rgb_out, uint32_t *img_out, void *cuda_array);
 
 #ifdef __cplusplus
 }
