@@ -331,10 +331,3 @@ class RenderCUDA:
     def assemble_rank(self, src_rank: int, world_size: int, accum_dev_ptr: int, img_dev_ptr: int) -> None:
         self._check(self.lib.crtc_assemble_rank(self.h, src_rank, world_size, C.c_void_p(accum_dev_ptr),
                                                 C.c_void_p(img_dev_ptr)))
-
-
-def local_tile_ids(fb_width: int, fb_height: int, rank: int, world_size: int):
-    """Tiles (64x64, ids as in render_embree.cpp:178-180) owned by ``rank``: id % world_size == rank."""
-    ntx = (fb_width + 63) // 64
-    nty = (fb_height + 63) // 64
-    return [t for t in range(ntx * nty) if t % world_size == rank]

@@ -5,7 +5,6 @@
 // frame, time it, read the framebuffer back. Everything per-frame runs on the GPU as the
 // kernel chain of kernels.cuh; there is no CPU fallback anywhere in this file.
 #include <algorithm>
-#include <chrono>
 #include <cmath>
 #include <cstdio>
 #include <memory>
@@ -137,7 +136,7 @@ struct crtc_renderer {
 
     // framebuffer layout
     int fb_w = 0, fb_h = 0;
-    uint32_t ntx = 0, nty = 0;
+    uint32_t ntx = 0;
     std::vector<uint32_t> local_tiles;
     uint32_t npx_local = 0;
     uint32_t frame_id = 0;
@@ -174,7 +173,7 @@ struct crtc_renderer {
         }
         std::vector<uchar4> rgba;
         for (uint32_t i = 0; i < scene->num_textures; ++i) {
-            const crt_image_t &im = scene->textures[i];  // (shape checked by convert_shading_inputs / flatten_scene)
+            const crt_image_t &im = scene->textures[i];  // (shape checked by pack_shading)
             const size_t n = (size_t)im.width * im.height;
             rgba.assign(n, make_uchar4(0, 0, 0, 0));  // channels the image lacks read as 0 (texture2d.ih:13-27)
             for (size_t px = 0; px < n; ++px) {
@@ -614,15 +613,8 @@ struct crtc_renderer {
         frame_id = 0;
         fb_w = w;
         fb_h = h;
-        // render_embree.cpp:43-44
-        ntx = w / crt::kTile + (w % crt::kTile != 0 ? 1 : 0);
-        nty = h / crt::kTile + (h % crt::kTile != 0 ? 1 : 0);
-        local_tiles.clear();
-        for (uint32_t t = 0; t < ntx * nty; ++t) {
-            if ((int)(t % (uint32_t)world_size) == rank) {
-                local_tiles.push_back(t);
-            }
-        }
+        ntx = crt::tiles_along(w);
+        local_tiles = crt::rank_tiles(w, h, rank, world_size);
         npx_local = (uint32_t)local_tiles.size() * crt::kTilePixels;
         assemble_tiles.clear();
         d_tile_ids.upload(local_tiles.data(), local_tiles.size(), stream);
@@ -646,15 +638,6 @@ struct crtc_renderer {
         CUDA_CHECK(cudaStreamSynchronize(stream));
     }
 
-    static void check_depth(uint32_t depth) { crt_host::check_bvh_depth(depth); }
-    // k_traverse packs a pooled (owner lane, leaf-order triangle index) pair into one 32-bit slot: 5 + 27 bits
-    static void check_triangle_count(size_t n)
-    {
-        if (n >= (size_t)crt::kMaxTriangles) {
-            throw std::runtime_error("set_scene: " + std::to_string(n) + " triangles; this backend holds at most 2^27 - 1 (" +
-                                     std::to_string(crt::kMaxTriangles - 1) + ") per scene");
-        }
-    }
     int builder_fallbacks = 0;  // device builds that fell back to the host builder (crtc_get_option "bvh_builder_fallbacks")
 
     void set_scene(const crt_scene_t *scene)
@@ -663,19 +646,18 @@ struct crtc_renderer {
         frame_id = 0;
         auto_frames = 0;
         auto_decided = false;
-        crt::HostScene hs;
+        crt::SceneRecords rec;  // the device build fills rec.shading only
         uint32_t bvh_nodes = 0, bvh_depth = 0;
         double bvh_ms = 0.0;
         size_t num_tris = 0;
         // (the plan is cheap — reference checks and counts — and gives the triangle total before anything is allocated)
         crt::FlattenPlan plan;
         crt::plan_flatten(scene, plan);
-        check_triangle_count(plan.total_tris);
+        crt::check_triangle_count(plan.total_tris);
         bool built_on_device = false;
         if (bvh_builder != 0 && plan.total_tris > 0) {
-            check_triangle_count(plan.total_tris);
             // set_scene on the device: only the references are checked and the materials / textures converted on the host
-            crt::convert_shading_inputs(scene, hs, bvh_threads);
+            crt::pack_shading(scene, bvh_threads, rec.shading);
             crt_host::DeviceSceneBuild job;
             job.stream = stream;
             job.device = device;
@@ -694,7 +676,6 @@ struct crtc_renderer {
                 // host builder takes over; scene errors and CUDA errors are not caught here
                 std::fprintf(stderr, "crt_cuda: %s; building the BVH on the host instead\n", e.what());
                 CUDA_CHECK(cudaStreamSynchronize(stream));
-                hs = crt::HostScene();
                 builder_fallbacks++;
             }
             if (built_on_device) {
@@ -709,59 +690,31 @@ struct crtc_renderer {
             }
         }
         if (!built_on_device) {
-            const auto t0 = std::chrono::steady_clock::now();
-            crt::flatten_scene(scene, hs, bvh_threads);
-            phase_ms[0] = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+            crt::pack_scene(scene, bvh_threads, rec);
+            phase_ms[0] = rec.flatten_ms;
             phase_ms[1] = phase_ms[2] = phase_ms[3] = 0.0;  // the host builder reports one figure: scene_info[3]
-            num_tris = hs.num_tris();
-            check_triangle_count(num_tris);
-            crt::Bvh8 bvh;
-            crt::build_bvh8(hs.tri_verts.data(), hs.num_tris(), bvh_threads, bvh);
-            check_depth(bvh.max_depth);
-            std::vector<float> tri_records;
-            std::vector<crt::TriShade> shade;
-            const auto t_pack = std::chrono::steady_clock::now();
-            crt::pack_triangles(hs, bvh, tri_records, shade, bvh_threads);
-            phase_ms[4] = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_pack).count();
-            leaf_flat_ids.resize(shade.size());
-            for (size_t i = 0; i < shade.size(); ++i) {
-                leaf_flat_ids[i] = shade[i].flat_id;
-            }
+            phase_ms[4] = rec.pack_ms;
+            num_tris = rec.num_tris;
+            leaf_flat_ids = std::move(rec.leaf_flat_ids);
             static_assert(sizeof(crt::Bvh8Node) == 5 * sizeof(float4), "node = 5 float4");
-            d_nodes.upload(reinterpret_cast<const float4 *>(bvh.nodes.data()), bvh.nodes.size() * 5, stream);
-            // keep at least one (degenerate) record so empty scenes have valid pointers
-            if (tri_records.empty()) {
-                tri_records.assign(12, 0.f);
-                shade.resize(1);
-                std::memset(&shade[0], 0, sizeof(crt::TriShade));
-            }
-            d_tris.upload(reinterpret_cast<const float4 *>(tri_records.data()), tri_records.size() / 4, stream);
-            d_shade.upload(reinterpret_cast<const float4 *>(shade.data()), shade.size() * 3, stream);
-            CUDA_CHECK(cudaStreamSynchronize(stream));  // the staging vectors go out of scope
-            bvh_nodes = (uint32_t)bvh.nodes.size();
-            bvh_depth = bvh.max_depth;
-            bvh_ms = bvh.build_seconds * 1e3;
+            d_nodes.upload(reinterpret_cast<const float4 *>(rec.bvh.nodes.data()), rec.bvh.nodes.size() * 5, stream);
+            d_tris.upload(reinterpret_cast<const float4 *>(rec.tris.data()), rec.tris.size() / 4, stream);
+            d_shade.upload(reinterpret_cast<const float4 *>(rec.shade.data()), rec.shade.size() * 3, stream);
+            bvh_nodes = (uint32_t)rec.bvh.nodes.size();
+            bvh_depth = rec.bvh.max_depth;
+            bvh_ms = rec.bvh.build_seconds * 1e3;
         }
+        const crt::ShadingRecords &sh = rec.shading;
         static_assert(sizeof(crt_material_t) == 64 && sizeof(crt_quad_light_t) == 80, "layouts");
-        if (hs.materials.empty()) {
-            hs.materials.resize(1);
-            std::memset(&hs.materials[0], 0, sizeof(crt_material_t));
-        }
-        d_materials.upload(reinterpret_cast<const float4 *>(hs.materials.data()), hs.materials.size() * 4, stream);
-        d_lights.upload(reinterpret_cast<const float4 *>(hs.lights.data()), hs.lights.size() * 5, stream);
-        num_lights = (uint32_t)hs.lights.size();
-        if (hs.texels.empty()) {
-            hs.texels.assign(1, 0u);
-        }
-        d_texels.upload(hs.texels.data(), hs.texels.size(), stream);
-        std::vector<crt::DevTex> tex(std::max<size_t>(1, hs.tex_desc.size()));
-        for (size_t i = 0; i < hs.tex_desc.size(); ++i) {
-            tex[i] = crt::DevTex{hs.tex_desc[i].offset, hs.tex_desc[i].width, hs.tex_desc[i].height, 0};
-        }
-        d_tex.upload(tex.data(), tex.size(), stream);
-        CUDA_CHECK(cudaStreamSynchronize(stream));
+        static_assert(sizeof(crt::TexDesc) == sizeof(crt::DevTex), "layouts");
+        d_materials.upload(reinterpret_cast<const float4 *>(sh.materials.data()), sh.materials.size() * 4, stream);
+        d_lights.upload(reinterpret_cast<const float4 *>(sh.lights.data()), sh.lights.size() * 5, stream);
+        num_lights = (uint32_t)sh.lights.size();
+        d_texels.upload(sh.texels.data(), sh.texels.size(), stream);
+        d_tex.upload(reinterpret_cast<const crt::DevTex *>(sh.tex_desc.data()), sh.tex_desc.size(), stream);
+        CUDA_CHECK(cudaStreamSynchronize(stream));  // (rec is the staging memory of every upload above)
         build_hw_textures(scene);
-        spp = std::max<uint32_t>(1u, hs.samples_per_pixel);
+        spp = sh.spp;
         have_scene = true;
         scene_info[0] = (double)num_tris;
         scene_info[1] = (double)bvh_nodes;
@@ -779,37 +732,6 @@ struct crtc_renderer {
                 CUDA_CHECK(cudaMemsetAsync(aov_state.local.ptr, 0, (size_t)npx_local * crt::kAovFloats * sizeof(float), stream));
             }
         }
-    }
-
-    static float3 glm_normalize(float3 v)
-    {
-        // glm::normalize(v) = v * inversesqrt(dot(v, v)), inversesqrt(x) = 1 / sqrt(x)
-        const float inv = 1.f / std::sqrt(v.x * v.x + v.y * v.y + v.z * v.z);
-        return make_float3(v.x * inv, v.y * inv, v.z * inv);
-    }
-    static float3 cross3(float3 a, float3 b)
-    {
-        return make_float3(a.y * b.z - b.y * a.z, a.z * b.x - b.z * a.x, a.x * b.y - b.x * a.y);
-    }
-
-    // render_embree.cpp:149-159 / render_optix.cpp:454-460
-    crt::ViewParams view_params(const float *pos, const float *dir_, const float *up_, float fovy) const
-    {
-        const float3 dir = make_float3(dir_[0], dir_[1], dir_[2]);
-        const float3 up = make_float3(up_[0], up_[1], up_[2]);
-        const float plane_y = 2.f * std::tan((0.5f * fovy) * 0.01745329251994329576923690768489f);
-        const float plane_x = plane_y * static_cast<float>(fb_w) / static_cast<float>(fb_h);
-        crt::ViewParams v;
-        v.pos = make_float3(pos[0], pos[1], pos[2]);
-        const float3 du = glm_normalize(cross3(dir, up));
-        v.dir_du = make_float3(du.x * plane_x, du.y * plane_x, du.z * plane_x);
-        const float3 dvn = glm_normalize(cross3(v.dir_du, dir));
-        v.dir_dv = make_float3(-dvn.x * plane_y, -dvn.y * plane_y, -dvn.z * plane_y);
-        v.dir_top_left = make_float3(dir.x - 0.5f * v.dir_du.x - 0.5f * v.dir_dv.x,
-                                     dir.y - 0.5f * v.dir_du.y - 0.5f * v.dir_dv.y,
-                                     dir.z - 0.5f * v.dir_du.z - 0.5f * v.dir_dv.z);
-        v.frame_id = frame_id;
-        return v;
     }
 
     // Enqueues one frame on the stream (no host synchronisation) and returns its record.
@@ -831,7 +753,7 @@ struct crtc_renderer {
         if (camera_changed) {
             frame_id = 0;  // render_embree.cpp:145-147
         }
-        const crt::ViewParams view = view_params(pos, dir, up, fovy);
+        const crt::ViewParams view = crt::make_view_params(pos, dir, up, fovy, fb_w, fb_h, frame_id);
         const size_t npaths = (size_t)npx_local * spp * num_frames;
         if (npaths >= 0x7fffffffull) {
             throw std::runtime_error("render: more than 2^31 paths in flight on one device");
@@ -1256,12 +1178,7 @@ struct crtc_renderer {
             }
         }
         if (!d_tiles) {
-            std::vector<uint32_t> tiles;
-            for (uint32_t t = 0; t < ntx * nty; ++t) {
-                if ((int)(t % (uint32_t)ws) == src_rank) {
-                    tiles.push_back(t);
-                }
-            }
+            const std::vector<uint32_t> tiles = crt::rank_tiles(fb_w, fb_h, src_rank, ws);
             assemble_tiles.emplace_back(key, std::make_unique<DeviceBuffer<uint32_t>>());
             d_tiles = assemble_tiles.back().second.get();
             d_tiles->upload(tiles.data(), tiles.size(), stream);

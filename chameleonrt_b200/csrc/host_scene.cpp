@@ -3,11 +3,12 @@
 // the values render_embree.ispc:269,288-290 would compute per hit.
 #include "host_scene.h"
 
-#include "bvh8.h"
+#include "bvh8_traverse.h"
 #include "host_parallel.h"
 
 #include <algorithm>
 #include <atomic>
+#include <chrono>
 #include <cmath>
 #include <cstring>
 #include <stdexcept>
@@ -15,6 +16,12 @@
 
 namespace crt {
 namespace {
+
+struct HostScene {
+    std::vector<float> tri_verts;  // 9 floats per triangle: v0, v1, v2 (world space)
+    std::vector<TriShade> tri_shade;
+    size_t num_tris() const { return tri_shade.size(); }
+};
 
 // 4x4 inverse by cofactor expansion, column-major (the role of glm::inverse in
 // embree_utils.cpp:97).
@@ -84,7 +91,28 @@ void check_param(float x, uint32_t num_textures, const char *what, uint32_t mat)
     }
 }
 
+double ms_since(std::chrono::steady_clock::time_point t0)
+{
+    return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+}
+
 }  // namespace
+
+// k_traverse packs a pooled (owner lane, leaf-order triangle index) pair into one 32-bit slot: 5 + 27 bits
+void check_triangle_count(size_t n)
+{
+    if (n >= (size_t)kMaxTriangles) {
+        throw std::runtime_error("set_scene: " + std::to_string(n) + " triangles; this backend holds at most 2^27 - 1 (" +
+                                 std::to_string(kMaxTriangles - 1) + ") per scene");
+    }
+}
+
+void check_bvh_depth(uint32_t depth)
+{
+    if (depth + 2 > CRT_STACK_SIZE) {
+        throw std::runtime_error("BVH8 depth " + std::to_string(depth) + " exceeds the traversal stack (CRT_STACK_SIZE)");
+    }
+}
 
 void plan_flatten(const crt_scene_t *s, FlattenPlan &plan)
 {
@@ -136,9 +164,12 @@ void plan_flatten(const crt_scene_t *s, FlattenPlan &plan)
     }
 }
 
+namespace {
+
+// The triangle half of the flattening; throws std::runtime_error on malformed input (bad material / mesh ids,
+// vertex indices out of range)
 void flatten_scene(const crt_scene_t *s, HostScene &out, int threads)
 {
-    out = HostScene();
     FlattenPlan plan;
     plan_flatten(s, plan);
     const size_t total = plan.total_tris;
@@ -219,12 +250,13 @@ void flatten_scene(const crt_scene_t *s, HostScene &out, int threads)
     if (bad_index) {
         throw std::runtime_error("triangle index out of range");
     }
-    convert_shading_inputs(s, out, threads);
 }
 
-void convert_shading_inputs(const crt_scene_t *s, HostScene &out, int threads)
+}  // namespace
+
+void pack_shading(const crt_scene_t *s, int threads, ShadingRecords &out)
 {
-    out.samples_per_pixel = s->samples_per_pixel;
+    out.spp = std::max<uint32_t>(1u, s->samples_per_pixel);
     // materials
     out.materials.assign(s->materials, s->materials + s->num_materials);
     for (uint32_t i = 0; i < s->num_materials; ++i) {
@@ -306,8 +338,22 @@ void convert_shading_inputs(const crt_scene_t *s, HostScene &out, int threads)
             out.texels[base + px] = (uint32_t)c[0] | ((uint32_t)c[1] << 8) | ((uint32_t)c[2] << 16) | ((uint32_t)c[3] << 24);
         }
     });
+    if (out.materials.empty()) {
+        out.materials.resize(1);
+        std::memset(&out.materials[0], 0, sizeof(crt_material_t));
+    }
+    if (out.texels.empty()) {
+        out.texels.assign(1, 0u);
+    }
+    if (out.tex_desc.empty()) {
+        out.tex_desc.assign(1, TexDesc{0, 0, 0, 0});
+    }
 }
 
+namespace {
+
+// Device-format triangle records in BVH leaf order (SceneRecords::tris), and the shading records permuted into the
+// same order.
 void pack_triangles(const HostScene &scene, const Bvh8 &bvh, std::vector<float> &tri_records,
                     std::vector<TriShade> &shade_leaf_order, int threads)
 {
@@ -337,6 +383,35 @@ void pack_triangles(const HostScene &scene, const Bvh8 &bvh, std::vector<float> 
         shade_leaf_order[i] = scene.tri_shade[src];
     }
     });
+}
+
+}  // namespace
+
+void pack_scene(const crt_scene_t *s, int threads, SceneRecords &out)
+{
+    out = SceneRecords();
+    HostScene hs;
+    const auto t0 = std::chrono::steady_clock::now();
+    flatten_scene(s, hs, threads);
+    pack_shading(s, threads, out.shading);
+    out.flatten_ms = ms_since(t0);
+    out.num_tris = hs.num_tris();
+    check_triangle_count(out.num_tris);
+    build_bvh8(hs.tri_verts.data(), hs.num_tris(), threads, out.bvh);
+    check_bvh_depth(out.bvh.max_depth);
+    const auto t_pack = std::chrono::steady_clock::now();
+    pack_triangles(hs, out.bvh, out.tris, out.shade, threads);
+    out.pack_ms = ms_since(t_pack);
+    out.leaf_flat_ids.resize(out.shade.size());
+    for (size_t i = 0; i < out.shade.size(); ++i) {
+        out.leaf_flat_ids[i] = out.shade[i].flat_id;
+    }
+    // keep at least one (degenerate) record so empty scenes have valid pointers
+    if (out.tris.empty()) {
+        out.tris.assign(12, 0.f);
+        out.shade.resize(1);
+        std::memset(&out.shade[0], 0, sizeof(TriShade));
+    }
 }
 
 }  // namespace crt

@@ -16,9 +16,13 @@
 #include <vector>
 
 #include "../../include/crt_scene.h"
+#include "bvh8.h"
 
 namespace crt {
 
+constexpr uint32_t kMaxTriangles = 1u << 27;  // k_traverse's pooled pairs: owner lane << 27 | leaf-order triangle index
+
+// The layout of DevTex (shade_math.cuh)
 struct TexDesc {
     uint32_t offset;  // first texel in the arena
     int32_t width, height;
@@ -35,31 +39,40 @@ struct TriShade {
 };
 static_assert(sizeof(TriShade) == 48, "TriShade is three float4");
 
-struct HostScene {
-    std::vector<float> tri_verts;   // 9 floats per triangle: v0, v1, v2 (world space)
-    std::vector<TriShade> tri_shade;
+// Materials, lights and the texture arena as set_scene uploads them. Every array but the lights holds at least one
+// element (zeros when the scene has none), so that the device always gets valid pointers.
+struct ShadingRecords {
     std::vector<crt_material_t> materials;
     std::vector<crt_quad_light_t> lights;
     std::vector<uint32_t> texels;  // RGBA8 arena
     std::vector<TexDesc> tex_desc;
-    uint32_t samples_per_pixel = 1;
-    size_t num_tris() const { return tri_shade.size(); }
+    uint32_t spp = 1;  // samples per pixel, at least 1
 };
 
-struct Bvh8;
+// Everything set_scene uploads when the BVH is built on the host, in device layout.
+struct SceneRecords {
+    Bvh8 bvh;  // bvh.nodes is the device node array (5 float4 per node)
+    // 12 floats per triangle in BVH leaf order: {v0.xyz, bits(flat id)}, {e1.xyz, 0}, {e2.xyz, 0} with
+    // e1 = v1 - v0, e2 = v2 - v0 (the subtraction the intersector would otherwise do per test)
+    std::vector<float> tris;
+    std::vector<TriShade> shade;  // the shading records in the same order
+    // tris and shade keep at least one (degenerate) record so empty scenes have valid pointers;
+    // leaf_flat_ids (leaf-order triangle -> flattened primitive id) has the real triangles only
+    std::vector<uint32_t> leaf_flat_ids;
+    ShadingRecords shading;
+    size_t num_tris = 0;
+    double flatten_ms = 0.0, pack_ms = 0.0;  // host wall clock of the flattening and of the leaf-order packing
+};
 
-// Device-format triangle records in BVH leaf order: 12 floats per triangle =
-// {v0.xyz, bits(flat id)}, {e1.xyz, 0}, {e2.xyz, 0} with e1 = v1 - v0, e2 = v2 - v0
-// (the subtraction the intersector would otherwise do per test), and the shading records
-// permuted into the same order.
-// threads <= 0: hardware concurrency.
-void pack_triangles(const HostScene &scene, const Bvh8 &bvh, std::vector<float> &tri_records,
-                    std::vector<TriShade> &shade_leaf_order, int threads = 0);
+// Flattens the scene, builds the BVH8 and packs the records. threads <= 0: hardware concurrency.
+// Throws std::runtime_error on malformed input (bad material / texture / mesh ids) and on scenes the kernels cannot
+// hold (check_triangle_count, check_bvh_depth).
+void pack_scene(const crt_scene_t *scene, int threads, SceneRecords &out);
 
-// Throws std::runtime_error on malformed input (bad material / texture / mesh ids).
-void flatten_scene(const crt_scene_t *scene, HostScene &out, int threads = 0);
+void check_triangle_count(size_t n);
+void check_bvh_depth(uint32_t depth);
 
-// The two halves of flatten_scene, for the device set_scene path (bvh8_device.cuh: k_flatten does the per-triangle
+// The two halves of the flattening, for the device set_scene path (bvh8_device.cuh: k_flatten does the per-triangle
 // work from the plan): (1) validation of the instance / mesh / material references, one segment per (instance,
 // geometry) with the index of its first flattened triangle, and every instance's world_to_object matrix
 // (embree_utils.cpp:97); (2) materials, lights and the texture arena (no triangles).
@@ -73,6 +86,6 @@ struct FlattenPlan {
     size_t total_tris = 0;
 };
 void plan_flatten(const crt_scene_t *scene, FlattenPlan &plan);
-void convert_shading_inputs(const crt_scene_t *scene, HostScene &out, int threads = 0);
+void pack_shading(const crt_scene_t *scene, int threads, ShadingRecords &out);
 
 }  // namespace crt

@@ -15,11 +15,7 @@
 
 namespace {
 struct HostCheck {
-    crt::HostScene scene;
-    crt::Bvh8 bvh;
-    std::vector<float> tri_records;
-    std::vector<crt::TriShade> shade;
-    std::vector<float> node_f4;
+    crt::SceneRecords rec;
 };
 std::string g_err;
 }  // namespace
@@ -35,11 +31,7 @@ void *crt_hostcheck_create(const crt_scene_t *scene, int threads)
 {
     try {
         auto *h = new HostCheck();
-        crt::flatten_scene(scene, h->scene, threads);
-        crt::build_bvh8(h->scene.tri_verts.data(), h->scene.num_tris(), threads, h->bvh);
-        crt::pack_triangles(h->scene, h->bvh, h->tri_records, h->shade, threads);
-        h->node_f4.resize(h->bvh.nodes.size() * 20);
-        std::memcpy(h->node_f4.data(), h->bvh.nodes.data(), h->bvh.nodes.size() * 80);
+        crt::pack_scene(scene, threads, h->rec);
         return h;
     } catch (const std::exception &e) {
         g_err = e.what();
@@ -56,11 +48,11 @@ void crt_hostcheck_destroy(void *p)
 void crt_hostcheck_stats(void *p, double *out5)
 {
     HostCheck *h = static_cast<HostCheck *>(p);
-    out5[0] = (double)h->bvh.nodes.size();
-    out5[1] = (double)h->bvh.tri_order.size();
-    out5[2] = (double)h->bvh.max_depth;
-    out5[3] = h->bvh.sah_cost;
-    out5[4] = h->bvh.build_seconds * 1e3;
+    out5[0] = (double)h->rec.bvh.nodes.size();
+    out5[1] = (double)h->rec.bvh.tri_order.size();
+    out5[2] = (double)h->rec.bvh.max_depth;
+    out5[3] = h->rec.bvh.sah_cost;
+    out5[4] = h->rec.bvh.build_seconds * 1e3;
 }
 
 // FNV-1a over the node array and the triangle order: lets tests assert that builder changes
@@ -75,8 +67,8 @@ uint64_t crt_hostcheck_digest(void *p)
             d = (d ^ b[i]) * 1099511628211ull;
         }
     };
-    mix(h->bvh.nodes.data(), h->bvh.nodes.size() * sizeof(crt::Bvh8Node));
-    mix(h->bvh.tri_order.data(), h->bvh.tri_order.size() * sizeof(uint32_t));
+    mix(h->rec.bvh.nodes.data(), h->rec.bvh.nodes.size() * sizeof(crt::Bvh8Node));
+    mix(h->rec.bvh.tri_order.data(), h->rec.bvh.tri_order.size() * sizeof(uint32_t));
     return d;
 }
 
@@ -86,8 +78,8 @@ void crt_hostcheck_trace(void *p, const float *rays, uint64_t n, int any_hit, fl
                          uint32_t *counters)
 {
     HostCheck *h = static_cast<HostCheck *>(p);
-    const float4 *nodes = reinterpret_cast<const float4 *>(h->node_f4.data());
-    const float4 *tris = reinterpret_cast<const float4 *>(h->tri_records.data());
+    const float4 *nodes = reinterpret_cast<const float4 *>(h->rec.bvh.nodes.data());
+    const float4 *tris = reinterpret_cast<const float4 *>(h->rec.tris.data());
     for (uint64_t i = 0; i < n; ++i) {
         crt::Ray r;
         std::memcpy(&r, rays + 8 * i, 32);
@@ -106,7 +98,7 @@ void crt_hostcheck_trace(void *p, const float *rays, uint64_t n, int any_hit, fl
         std::memcpy(&o[3], &hit.flat, 4);
         if (normals) {
             for (int k = 0; k < 3; ++k) {
-                normals[3 * i + k] = hit.tri == 0xffffffffu ? 0.f : h->shade[hit.tri].n[k];
+                normals[3 * i + k] = hit.tri == 0xffffffffu ? 0.f : h->rec.shade[hit.tri].n[k];
             }
         }
         if (counters) {

@@ -18,7 +18,9 @@
 // the traversal uses explicit fma (bvh8_traverse.h).
 #pragma once
 
+#include <cmath>
 #include <cstdint>
+#include <vector>
 #include <cuda_runtime.h>
 
 #include "bvh8_traverse.h"
@@ -30,7 +32,6 @@ constexpr uint32_t kMiss = 0xffffffffu;
 constexpr int kTile = 64;                 // render_embree.h:25
 constexpr uint32_t kTilePixels = kTile * kTile;
 constexpr int kMaxDepthSupported = 16;
-constexpr uint32_t kMaxTriangles = 1u << 27;  // k_traverse's pooled pairs: owner lane << 27 | leaf-order triangle index
 // counters layout (uint32): [0..16] queue length entering bounce b; [17..33] shadow rays
 // emitted at bounce b; [34] paths started
 constexpr int kCntQueue = 0;
@@ -43,6 +44,51 @@ struct ViewParams {
     float3 pos, dir_du, dir_dv, dir_top_left;  // embree_utils.h:137-140
     uint32_t frame_id;
 };
+
+// The camera basis on the host, render_embree.cpp:149-159 / render_optix.cpp:454-460. Its callers are compiled with
+// -ffp-contract=off, so that the basis is the reference's to the bit.
+inline ViewParams make_view_params(const float *pos, const float *dir_, const float *up_, float fovy, int fb_w, int fb_h,
+                                   uint32_t frame_id)
+{
+    // glm::normalize(v) = v * inversesqrt(dot(v, v)), inversesqrt(x) = 1 / sqrt(x)
+    const auto glm_normalize = [](float3 v) {
+        const float inv = 1.f / std::sqrt(v.x * v.x + v.y * v.y + v.z * v.z);
+        return make_float3(v.x * inv, v.y * inv, v.z * inv);
+    };
+    const auto cross3 = [](float3 a, float3 b) {
+        return make_float3(a.y * b.z - b.y * a.z, a.z * b.x - b.z * a.x, a.x * b.y - b.x * a.y);
+    };
+    const float3 dir = make_float3(dir_[0], dir_[1], dir_[2]);
+    const float3 up = make_float3(up_[0], up_[1], up_[2]);
+    const float plane_y = 2.f * std::tan((0.5f * fovy) * 0.01745329251994329576923690768489f);
+    const float plane_x = plane_y * static_cast<float>(fb_w) / static_cast<float>(fb_h);
+    ViewParams v;
+    v.pos = make_float3(pos[0], pos[1], pos[2]);
+    const float3 du = glm_normalize(cross3(dir, up));
+    v.dir_du = make_float3(du.x * plane_x, du.y * plane_x, du.z * plane_x);
+    const float3 dvn = glm_normalize(cross3(v.dir_du, dir));
+    v.dir_dv = make_float3(-dvn.x * plane_y, -dvn.y * plane_y, -dvn.z * plane_y);
+    v.dir_top_left = make_float3(dir.x - 0.5f * v.dir_du.x - 0.5f * v.dir_dv.x,
+                                 dir.y - 0.5f * v.dir_du.y - 0.5f * v.dir_dv.y,
+                                 dir.z - 0.5f * v.dir_du.z - 0.5f * v.dir_dv.z);
+    v.frame_id = frame_id;
+    return v;
+}
+
+// Tiles along a framebuffer side of n pixels (render_embree.cpp:43-44)
+inline uint32_t tiles_along(int n) { return n / kTile + (n % kTile != 0 ? 1 : 0); }
+
+// The row-major ids of the tiles that rank `rank` of `world` renders: every world-th tile, starting at its own rank
+inline std::vector<uint32_t> rank_tiles(int w, int h, int rank, int world)
+{
+    std::vector<uint32_t> tiles;
+    for (uint32_t t = 0; t < tiles_along(w) * tiles_along(h); ++t) {
+        if ((int)(t % (uint32_t)world) == rank) {
+            tiles.push_back(t);
+        }
+    }
+    return tiles;
+}
 
 struct DeviceScene {
     const float4 *nodes;      // 5 per BVH8 node

@@ -46,13 +46,6 @@ struct EventSet {
     cudaEvent_t operator[](size_t i) const { return ev[i]; }
 };
 
-inline void check_bvh_depth(uint32_t depth)
-{
-    if (depth + 2 > CRT_STACK_SIZE) {
-        throw std::runtime_error("BVH8 depth " + std::to_string(depth) + " exceeds the traversal stack (CRT_STACK_SIZE)");
-    }
-}
-
 struct DeviceSceneBuild {
     // in
     cudaStream_t stream = nullptr;

@@ -30,8 +30,7 @@ namespace {
 std::string g_err;
 
 struct SimtCheck {
-    std::vector<float4> nodes, tris;
-    std::vector<uint32_t> leaf_flat_ids;  // leaf-order triangle index -> flattened primitive id
+    crt::SceneRecords rec;
 };
 
 }  // namespace
@@ -44,23 +43,7 @@ void *crt_simt_create(const crt_scene_t *scene)
 {
     try {
         auto *h = new SimtCheck();
-        crt::HostScene hs;
-        crt::flatten_scene(scene, hs, 0);
-        crt::Bvh8 bvh;
-        crt::build_bvh8(hs.tri_verts.data(), hs.num_tris(), 0, bvh);
-        std::vector<float> rec;
-        std::vector<crt::TriShade> sh;
-        crt::pack_triangles(hs, bvh, rec, sh, 0);
-        h->nodes.resize(bvh.nodes.size() * 5);
-        std::memcpy(h->nodes.data(), bvh.nodes.data(), bvh.nodes.size() * 80);
-        if (rec.empty()) {
-            rec.assign(12, 0.f);
-        }
-        h->tris.resize(rec.size() / 4);
-        std::memcpy(h->tris.data(), rec.data(), rec.size() * 4);
-        for (const crt::TriShade &t : sh) {
-            h->leaf_flat_ids.push_back(t.flat_id);
-        }
+        crt::pack_scene(scene, 0, h->rec);
         return h;
     } catch (const std::exception &e) {
         g_err = e.what();
@@ -115,8 +98,8 @@ void crt_simt_traverse(void *p, const float *closest, uint32_t n_closest, const 
     counters[crt::kCntQueue] = n_closest;
     counters[crt::kCntShadow] = n_any;
     crt::DeviceScene sc{};
-    sc.nodes = h->nodes.data();
-    sc.tris = h->tris.data();
+    sc.nodes = reinterpret_cast<const float4 *>(h->rec.bvh.nodes.data());
+    sc.tris = reinterpret_cast<const float4 *>(h->rec.tris.data());
     sc.float_one = 0x3F800000u;
     crt::PathState ps{};
     ps.ray_o = ray_o.data();
@@ -166,7 +149,8 @@ void crt_simt_traverse(void *p, const float *closest, uint32_t n_closest, const 
         hits_out[4 * i + 1] = hit[i].y;
         hits_out[4 * i + 2] = hit[i].z;
         const uint32_t leaf = __float_as_uint(hit[i].w);
-        hits_out[4 * i + 3] = __uint_as_float(leaf == crt::kMiss || leaf >= h->leaf_flat_ids.size() ? crt::kMiss : h->leaf_flat_ids[leaf]);
+        const std::vector<uint32_t> &flat_ids = h->rec.leaf_flat_ids;
+        hits_out[4 * i + 3] = __uint_as_float(leaf == crt::kMiss || leaf >= flat_ids.size() ? crt::kMiss : flat_ids[leaf]);
     }
     if (n_any) {
         std::memcpy(vis_out, vis.data(), n_any);

@@ -104,11 +104,8 @@ namespace {
 std::string g_err;
 
 struct HostWavefront {
-    // scene (device-format records, host memory)
-    std::vector<float4> nodes, tris, shade, materials, lights;
-    std::vector<uint32_t> texels;
-    std::vector<crt::DevTex> tex;
-    uint32_t num_lights = 0, spp = 1;
+    crt::SceneRecords rec;  // the scene in device layout, host memory
+    uint32_t spp = 1;
     // framebuffer
     int fb_w = 0, fb_h = 0;
     uint32_t ntx = 0, npx_local = 0;
@@ -128,57 +125,23 @@ struct HostWavefront {
     crt::DeviceScene device_scene() const
     {
         crt::DeviceScene sc;
-        sc.nodes = nodes.data();
-        sc.tris = tris.data();
-        sc.shade = shade.data();
-        sc.materials = materials.data();
-        sc.lights = lights.data();
-        sc.texels = texels.data();
-        sc.tex = tex.data();
-        sc.num_lights = num_lights;
+        sc.nodes = reinterpret_cast<const float4 *>(rec.bvh.nodes.data());
+        sc.tris = reinterpret_cast<const float4 *>(rec.tris.data());
+        sc.shade = reinterpret_cast<const float4 *>(rec.shade.data());
+        sc.materials = reinterpret_cast<const float4 *>(rec.shading.materials.data());
+        sc.lights = reinterpret_cast<const float4 *>(rec.shading.lights.data());
+        sc.texels = rec.shading.texels.data();
+        sc.tex = reinterpret_cast<const crt::DevTex *>(rec.shading.tex_desc.data());
+        sc.num_lights = (uint32_t)rec.shading.lights.size();
         sc.float_one = 0x3F800000u;
         return sc;
     }
 
     void set_scene(const crt_scene_t *scene)
     {
-        // crtc_renderer::set_scene
-        crt::HostScene hs;
-        crt::flatten_scene(scene, hs, 0);
-        crt::Bvh8 bvh;
-        crt::build_bvh8(hs.tri_verts.data(), hs.num_tris(), 0, bvh);
-        std::vector<float> tri_records;
-        std::vector<crt::TriShade> sh;
-        crt::pack_triangles(hs, bvh, tri_records, sh, 0);
-        nodes.resize(bvh.nodes.size() * 5);
-        std::memcpy(nodes.data(), bvh.nodes.data(), bvh.nodes.size() * 80);
-        if (tri_records.empty()) {
-            tri_records.assign(12, 0.f);
-            sh.resize(1);
-            std::memset(&sh[0], 0, sizeof(crt::TriShade));
-        }
-        tris.resize(tri_records.size() / 4);
-        std::memcpy(tris.data(), tri_records.data(), tri_records.size() * 4);
-        shade.resize(sh.size() * 3);
-        std::memcpy(shade.data(), sh.data(), sh.size() * sizeof(crt::TriShade));
-        if (hs.materials.empty()) {
-            hs.materials.resize(1);
-            std::memset(&hs.materials[0], 0, sizeof(crt_material_t));
-        }
-        materials.resize(hs.materials.size() * 4);
-        std::memcpy(materials.data(), hs.materials.data(), hs.materials.size() * 64);
-        lights.resize(hs.lights.size() * 5);
-        std::memcpy(lights.data(), hs.lights.data(), hs.lights.size() * 80);
-        num_lights = (uint32_t)hs.lights.size();
-        texels.assign(hs.texels.begin(), hs.texels.end());
-        if (texels.empty()) {
-            texels.assign(1, 0u);
-        }
-        tex.assign(std::max<size_t>(1, hs.tex_desc.size()), crt::DevTex{0, 0, 0, 0});
-        for (size_t i = 0; i < hs.tex_desc.size(); ++i) {
-            tex[i] = crt::DevTex{hs.tex_desc[i].offset, hs.tex_desc[i].width, hs.tex_desc[i].height, 0};
-        }
-        spp = std::max<uint32_t>(1u, hs.samples_per_pixel);
+        // crtc_renderer::set_scene: the kernels read the records where pack_scene left them
+        crt::pack_scene(scene, 0, rec);
+        spp = rec.shading.spp;
         frame_id = 0;
         std::fill(accum_local.begin(), accum_local.end(), 0.f);
     }
@@ -189,47 +152,13 @@ struct HostWavefront {
         fb_w = w;
         fb_h = h;
         frame_id = 0;
-        ntx = w / crt::kTile + (w % crt::kTile != 0 ? 1 : 0);
-        const uint32_t nty = h / crt::kTile + (h % crt::kTile != 0 ? 1 : 0);
-        tile_ids.clear();
-        for (uint32_t t = 0; t < ntx * nty; ++t) {
-            if ((int)(t % (uint32_t)world) == rank) {
-                tile_ids.push_back(t);
-            }
-        }
+        ntx = crt::tiles_along(w);
+        tile_ids = crt::rank_tiles(w, h, rank, world);
         npx_local = (uint32_t)tile_ids.size() * crt::kTilePixels;
         accum_local.assign((size_t)npx_local * 3, 0.f);
         img_local.assign(npx_local, 0u);
         accum_full.assign((size_t)w * h * 3, 0.f);
         img_full.assign((size_t)w * h, 0u);
-    }
-
-    static float3 glm_normalize(float3 v)
-    {
-        const float inv = 1.f / std::sqrt(v.x * v.x + v.y * v.y + v.z * v.z);
-        return make_float3(v.x * inv, v.y * inv, v.z * inv);
-    }
-    static float3 cross3(float3 a, float3 b)
-    {
-        return make_float3(a.y * b.z - b.y * a.z, a.z * b.x - b.z * a.x, a.x * b.y - b.x * a.y);
-    }
-    // crtc_renderer::view_params
-    crt::ViewParams view_params(const float *pos, const float *dir_, const float *up_, float fovy) const
-    {
-        const float3 dir = make_float3(dir_[0], dir_[1], dir_[2]);
-        const float3 up = make_float3(up_[0], up_[1], up_[2]);
-        const float plane_y = 2.f * std::tan((0.5f * fovy) * 0.01745329251994329576923690768489f);
-        const float plane_x = plane_y * static_cast<float>(fb_w) / static_cast<float>(fb_h);
-        crt::ViewParams v;
-        v.pos = make_float3(pos[0], pos[1], pos[2]);
-        const float3 du = glm_normalize(cross3(dir, up));
-        v.dir_du = make_float3(du.x * plane_x, du.y * plane_x, du.z * plane_x);
-        const float3 dvn = glm_normalize(cross3(v.dir_du, dir));
-        v.dir_dv = make_float3(-dvn.x * plane_y, -dvn.y * plane_y, -dvn.z * plane_y);
-        v.dir_top_left = make_float3(dir.x - 0.5f * v.dir_du.x - 0.5f * v.dir_dv.x, dir.y - 0.5f * v.dir_du.y - 0.5f * v.dir_dv.y,
-                                     dir.z - 0.5f * v.dir_du.z - 0.5f * v.dir_dv.z);
-        v.frame_id = frame_id;
-        return v;
     }
 
     template <typename F>
@@ -247,11 +176,12 @@ struct HostWavefront {
     // the work of one k_traverse launch: shadow rays [0, n_any) then closest-hit rays through `queue`
     void traverse(const crt::PathState &ps, const uint32_t *queue, uint32_t n_closest, uint32_t n_any, bool far_first)
     {
+        const crt::DeviceScene sc = device_scene();
         for (uint32_t j = 0; j < n_any; ++j) {
             const float4 o = ps.sray_o[j], d = ps.sray_d[j];
             const crt::Ray ray{o.x, o.y, o.z, crt::kEpsilon, d.x, d.y, d.z, o.w};
             crt::HitRecord h;
-            crt::bvh8_trace<true, false>(nodes.data(), tris.data(), ray, h, nullptr, far_first);
+            crt::bvh8_trace<true, false>(sc.nodes, sc.tris, ray, h, nullptr, far_first);
             ps.vis[__float_as_uint(d.w)] = h.tri != crt::kMiss ? 0 : 1;
         }
         for (uint32_t j = 0; j < n_closest; ++j) {
@@ -259,7 +189,7 @@ struct HostWavefront {
             const float4 o = ps.ray_o[slot], d = ps.ray_d[slot];
             const crt::Ray ray{o.x, o.y, o.z, o.w, d.x, d.y, d.z, d.w};
             crt::HitRecord h;
-            crt::bvh8_trace<false, false>(nodes.data(), tris.data(), ray, h, nullptr);
+            crt::bvh8_trace<false, false>(sc.nodes, sc.tris, ray, h, nullptr);
             const bool hit = h.tri != crt::kMiss;
             ps.hit[slot] = make_float4(h.t, hit ? h.u : 0.f, hit ? h.v : 0.f, __uint_as_float(h.tri));
         }
@@ -272,7 +202,7 @@ struct HostWavefront {
         if (camera_changed) {
             frame_id = 0;
         }
-        const crt::ViewParams view = view_params(pos, dir, up, fovy);
+        const crt::ViewParams view = crt::make_view_params(pos, dir, up, fovy, fb_w, fb_h, frame_id);
         const size_t npaths = (size_t)npx_local * spp * num_frames;
         for (auto *v : {&ray_o, &ray_d, &hit, &thr_rng, &radiance, &nee_T, &nee_l1, &nee_l2}) {
             v->assign(npaths, make_float4(0.f, 0.f, 0.f, 0.f));

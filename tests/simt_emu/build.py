@@ -42,7 +42,7 @@ def translate(src: str, expected: int) -> str:
 
 def build(force: bool = False) -> str:
     srcs = [os.path.join(CSRC, f) for f in ("crt_cuda_core.cu", "scene_device_build.cuh", "cuda_host_utils.h", "bvh8_device.cuh", "kernels.cuh", "shade_math.cuh", "bvh8_traverse.h", "simt_env.h",
-                                            "host_scene.cpp", "bvh8_build.cpp")] + [os.path.join(HERE, "cuda_emu.cpp"), __file__]
+                                            "host_scene.h", "host_scene.cpp", "bvh8.h", "bvh8_build.cpp")] + [os.path.join(HERE, "cuda_emu.cpp"), __file__]
     if not force and os.path.exists(LIB) and all(os.path.getmtime(LIB) >= os.path.getmtime(s) for s in srcs):
         return LIB
     os.makedirs(OUT, exist_ok=True)
