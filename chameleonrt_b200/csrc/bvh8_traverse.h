@@ -100,12 +100,17 @@ CRT_HD float fma_(float a, float b, float c)
 #endif
 }
 // 1 / x for the box test only (|x| >= 1e-20, so neither the input nor the result is subnormal)
+// CRT_RCP_SKEW (host builds of the host checks only): -1 moves the exact reciprocal one ulp towards zero, +1 one ulp away
+// from it, so that the box test's slack for the error of the device's approximate reciprocal is tested off the GPU.
 CRT_HD float rcp_box(float x)
 {
 #if defined(__CUDA_ARCH__)
     float r;
     asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
     return r;
+#elif defined(CRT_RCP_SKEW)
+    const float r = 1.f / x;
+    return nextafterf(r, CRT_RCP_SKEW < 0 ? 0.f : copysignf(INFINITY, r));
 #else
     return 1.f / x;
 #endif

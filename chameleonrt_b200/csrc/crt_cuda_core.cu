@@ -1059,27 +1059,37 @@ struct crtc_renderer {
         if (n > 0x3fffffffull) {
             throw std::runtime_error("trace_any: too many rays in one batch");
         }
-        ensure_path_buffers(std::max<size_t>((n + 1) / 2, path_capacity));
-        // the any-hit kernel uses tnear = EPSILON like the reference's shadow rays; a batch ray
-        // with another tnear is moved along its direction so the interval is preserved
-        std::vector<float> adj(rays, rays + 8 * n);
+        // The any-hit kernel starts every ray at tnear = kEpsilon, like the renderer's shadow rays. A ray with any other
+        // tnear goes through the closest-hit kernel instead: over the same triangle test, "occluded" is "a hit was found".
+        std::vector<float> any_rays, closest_rays;
+        std::vector<uint64_t> any_index, closest_index;
         for (uint64_t i = 0; i < n; ++i) {
-            const float shift = adj[8 * i + 3] - crt::kEpsilon;
-            if (shift != 0.f) {
-                for (int k = 0; k < 3; ++k) {
-                    adj[8 * i + k] += shift * adj[8 * i + 4 + k];
-                }
-                adj[8 * i + 7] -= shift;
+            const bool any_kernel = rays[8 * i + 3] == crt::kEpsilon;
+            std::vector<float> &dst = any_kernel ? any_rays : closest_rays;
+            dst.insert(dst.end(), rays + 8 * i, rays + 8 * i + 8);
+            (any_kernel ? any_index : closest_index).push_back(i);
+        }
+        if (!any_index.empty()) {
+            const uint64_t m = any_index.size();
+            ensure_path_buffers(std::max<size_t>((m + 1) / 2, path_capacity));
+            stage_any(m, any_rays.data());
+            launch_any(m);
+            std::vector<uint8_t> vis(m);
+            CUDA_CHECK(cudaMemcpyAsync(vis.data(), d_vis.ptr, m, cudaMemcpyDeviceToHost, stream));
+            CUDA_CHECK(cudaStreamSynchronize(stream));
+            CUDA_CHECK(cudaGetLastError());
+            for (uint64_t j = 0; j < m; ++j) {
+                occluded[any_index[j]] = vis[j] ? 0 : 1;
             }
         }
-        stage_any(n, adj.data());
-        launch_any(n);
-        std::vector<uint8_t> vis(n);
-        CUDA_CHECK(cudaMemcpyAsync(vis.data(), d_vis.ptr, n, cudaMemcpyDeviceToHost, stream));
-        CUDA_CHECK(cudaStreamSynchronize(stream));
-        CUDA_CHECK(cudaGetLastError());
-        for (uint64_t i = 0; i < n; ++i) {
-            occluded[i] = vis[i] ? 0 : 1;
+        if (!closest_index.empty()) {
+            std::vector<float> hits(4 * closest_index.size());
+            trace_closest(closest_rays.data(), closest_index.size(), hits.data());
+            for (uint64_t j = 0; j < closest_index.size(); ++j) {
+                uint32_t flat;
+                std::memcpy(&flat, &hits[4 * j + 3], 4);
+                occluded[closest_index[j]] = flat != crt::kMiss ? 1 : 0;
+            }
         }
     }
 

@@ -232,6 +232,21 @@ constexpr uint32_t kFetchBatch = 64;
 // north_star asks for BVH nodes staged in shared memory; measured on an H100 SXM it does not pay (frame +2-3 % on C2 / C4):
 // those nodes are the hottest lines of the L1 anyway and the copy takes 5.8 KB per block = 47 KB of L1 per SM away.
 constexpr uint32_t kTopNodes = 73;
+
+// The hit merge of k_traverse takes the 64-bit minimum of hit_key(t) << 32 | flat id. hit_key is monotone over every
+// float t (a negative t has all bits flipped, a non-negative one only its sign bit), so hits behind the origin of a ray
+// with tnear < 0 (crtc_trace_closest) merge like any other. -0 takes the key of +0: test_next_triangle treats them as
+// equal and breaks the tie on the flat id. hit_key_t inverts the map (giving +0 for either zero).
+__device__ __forceinline__ uint32_t hit_key(float t)
+{
+    const uint32_t u = f2u(t + 0.f);  // -0 + 0 = +0; every other t is unchanged
+    return u ^ ((uint32_t)((int32_t)u >> 31) | 0x80000000u);
+}
+__device__ __forceinline__ float hit_key_t(uint32_t k)
+{
+    return u2f(k ^ ((uint32_t)((int32_t)~k >> 31) | 0x80000000u));
+}
+
 template <bool COUNT, int DEFER = 0, bool TOP = false>
 __global__ void __launch_bounds__(kTravBlock, 8)
     k_traverse(DeviceScene sc, PathState ps, const uint32_t *queue, const uint32_t *count_closest_ptr,
@@ -252,8 +267,8 @@ __global__ void __launch_bounds__(kTravBlock, 8)
     // warp-cooperative triangle testing: per warp, every lane's ray and best hit live in
     // shared memory so that ANY lane can test a (ray, triangle) pair for its owner
     __shared__ float sm_ray[kTravBlock / 32][8][32];            // ox oy oz tnear dx dy dz tfar0
-    __shared__ unsigned long long sm_key[kTravBlock / 32][32];  // bits(t) << 32 | flat id  (atomicMin)
-    __shared__ float4 sm_hit[kTravBlock / 32][32];              // u, v, bits(leaf-order triangle | kMiss) of the best hit: one 128-bit store
+    __shared__ unsigned long long sm_key[kTravBlock / 32][32];  // hit_key(t) << 32 | flat id  (atomicMin)
+    __shared__ float4 sm_hit[kTravBlock / 32][32];              // u, v, bits(leaf-order triangle | kMiss), t of the best hit: one 128-bit store
     __shared__ uint32_t sm_owner[kTravBlock / 32][32];          // owner lane of the group that starts at slot s
     __shared__ uint32_t sm_cursor[kTravBlock / 32];             // running slot cursor of the warp (never reset)
     __shared__ uint32_t sm_is_any[kTravBlock / 32][32];         // ray kind per lane (instrumented build only)
@@ -331,8 +346,8 @@ __global__ void __launch_bounds__(kTravBlock, 8)
                     sm_ray[warp][5][lane] = ray.dy;
                     sm_ray[warp][6][lane] = ray.dz;
                     sm_ray[warp][7][lane] = ray.tfar;
-                    sm_key[warp][lane] = ((unsigned long long)__float_as_uint(ray.tfar) << 32) | 0xffffffffull;
-                    sm_hit[warp][lane] = make_float4(0.f, 0.f, __uint_as_float(kMiss), 0.f);
+                    sm_key[warp][lane] = ((unsigned long long)hit_key(ray.tfar) << 32) | 0xffffffffull;
+                    sm_hit[warp][lane] = make_float4(0.f, 0.f, __uint_as_float(kMiss), ray.tfar);
                     if (COUNT) {
                         sm_is_any[warp][lane] = is_any ? 1u : 0u;
                     }
@@ -446,7 +461,7 @@ __global__ void __launch_bounds__(kTravBlock, 8)
                     bool won = false;
                     unsigned long long cand = 0ull;
                     uint32_t tri_index = 0u;
-                    float hu = 0.f, hv = 0.f;
+                    float hu = 0.f, hv = 0.f, t = 0.f;
                     if ((uint32_t)lane < npairs) {
                         // the rank-th highest set bit of the group: two predicated steps cover a leaf (<= 3 triangles)
                         uint32_t skip = rank;
@@ -481,15 +496,14 @@ __global__ void __launch_bounds__(kTravBlock, 8)
                         r.tfar = sm_ray[warp][7][owner];
                         const float4 *tp = sc.tris + (size_t)tri_index * 3;
                         const float4 t0 = tp[0], t1 = tp[1], t2 = tp[2];
-                        float t;
                         if (tri_test(r, r.tfar, t0, t1, t2, t, hu, hv)) {
-                            cand = ((unsigned long long)__float_as_uint(t) << 32) | (unsigned long long)__float_as_uint(t0.w);
+                            cand = ((unsigned long long)hit_key(t) << 32) | (unsigned long long)__float_as_uint(t0.w);
                             won = atomicMin(&sm_key[warp][owner], cand) > cand;
                         }
                     }
                     __syncwarp();
-                    if (won && sm_key[warp][owner] == cand) {  // the pair that holds the minimum records u, v
-                        sm_hit[warp][owner] = make_float4(hu, hv, __uint_as_float(tri_index), 0.f);
+                    if (won && sm_key[warp][owner] == cand) {  // the pair that holds the minimum records u, v and its own t (-0 or +0)
+                        sm_hit[warp][owner] = make_float4(hu, hv, __uint_as_float(tri_index), t);
                     }
                     __syncwarp();
                     if (total <= 32u) {
@@ -498,7 +512,7 @@ __global__ void __launch_bounds__(kTravBlock, 8)
                 }
                 // refresh tfar, pop, finish
                 if (alive) {
-                    st.tfar = __uint_as_float((uint32_t)(sm_key[warp][lane] >> 32));
+                    st.tfar = hit_key_t((uint32_t)(sm_key[warp][lane] >> 32));
                     bool finished = is_any && __float_as_uint(sm_hit[warp][lane].z) != kMiss;
                     if (DEFER > 0 && finished) {
                         tri.y = 0u;  // an occluded shadow ray needs no further tests
@@ -517,8 +531,7 @@ __global__ void __launch_bounds__(kTravBlock, 8)
                         if (is_any) {
                             ps.vis[out_index] = htri != kMiss ? 0 : 1;
                         } else {
-                            ps.hit[out_index] = make_float4(__uint_as_float((uint32_t)(sm_key[warp][lane] >> 32)),
-                                                            htri != kMiss ? best.x : 0.f, htri != kMiss ? best.y : 0.f,
+                            ps.hit[out_index] = make_float4(best.w, htri != kMiss ? best.x : 0.f, htri != kMiss ? best.y : 0.f,
                                                             __uint_as_float(htri));
                         }
                         alive = false;

@@ -179,7 +179,10 @@ int crtc_get_scene_info(crtc_renderer *r, double *out, int n);
 /* Kernel-level access for parity tests and micro-benchmarks: trace a batch of rays against
  * the current scene with the same traversal kernels render() uses. rays: n*8 floats
  * {ox,oy,oz,tnear,dx,dy,dz,tfar} in HOST memory; hits: n*4 floats {t,u,v,bits(flat prim id or
- * 0xffffffff)}; occluded: n bytes. */
+ * 0xffffffff)}; occluded: n bytes. A hit is a triangle at tnear < t < tfar, for any tnear, negative included (t < 0 is
+ * a hit behind the origin); ties in t (-0 == +0) go to the lower primitive id, and a miss reports t = tfar. In
+ * crtc_trace_any, rays whose tnear is exactly 1e-4f (the renderer's shadow rays) run the any-hit kernel; every other
+ * ray runs the closest-hit kernel and is occluded when it finds a hit. Both answer for the ray's own interval. */
 int crtc_trace_closest(crtc_renderer *r, const float *rays, uint64_t n, float *hits);
 int crtc_trace_any(crtc_renderer *r, const float *rays, uint64_t n, uint8_t *occluded);
 /* Same kernels on DEVICE-resident rays, repeated `iters` times, returning the mean kernel time

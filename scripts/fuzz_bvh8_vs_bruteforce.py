@@ -5,7 +5,8 @@ vertices, huge + tiny triangles in one scene; rays from random points, from poin
 rays with exactly zero components travelling along grid lines, short shadow-ray segments. Closest hits must be
 bit-identical (t, u, v, primitive id), occlusion answers equal. CPU only.
 With --device the same scenes and rays also go through the DEVICE builders (bvh8_device.cuh: PLOC and LBVH, run under
-the SIMT emulation of tests/simt_emu) and the production traversal kernel over their trees: same hits, bit for bit.
+the SIMT emulation of tests/simt_emu) and the production traversal kernel over their trees: same closest hits, bit for
+bit, and the same occlusion answers as brute force.
     python scripts/fuzz_bvh8_vs_bruteforce.py [n] [first_seed] [--device]"""
 import os
 import sys
@@ -74,76 +75,74 @@ def random_rays(rng, scene, n):
     return np.ascontiguousarray(np.concatenate([o, tnear[:, None], d, tfar[:, None]], 1), np.float32)
 
 
+def scene_of(geoms):
+    """A one-mesh, identity-instanced scene of the given geometries."""
+    return Scene(meshes=[Mesh(geoms)], parameterized_meshes=[ParameterizedMesh(0, [0] * len(geoms))],
+                 instances=[Instance(np.eye(4, dtype=np.float32), 0)], materials=[DisneyMaterial()], textures=[],
+                 lights=[default_obj_light()], samples_per_pixel=1)
+
+
+def without_needles(scene):
+    """``scene`` with its needle triangles (2 * area / longest edge^2 < 1e-2) removed, as one geometry; the scene itself
+    if it has none. Needles are ill-conditioned for the triangle formula itself: the computed t can be off by far more
+    than rounding (seed 98: a 0.04-long sliver 800 units away "hit" at t = 800.911 while its box spans
+    [800.939, 800.943]), so no hierarchy can agree with brute force on them."""
+    tris = np.concatenate([np.asarray(g.vertices, np.float32)[np.asarray(g.indices, np.uint32).reshape(-1, 3)]
+                           for g in scene.meshes[0].geometries]).astype(np.float64)
+    e = [tris[:, 1] - tris[:, 0], tris[:, 2] - tris[:, 0], tris[:, 2] - tris[:, 1]]
+    longest = np.maximum(np.maximum((e[0] ** 2).sum(1), (e[1] ** 2).sum(1)), (e[2] ** 2).sum(1))
+    quality = np.linalg.norm(np.cross(e[0], e[1]), axis=1) / np.maximum(longest, 1e-300)
+    if not (quality < 1e-2).any():
+        return scene
+    kept = tris[quality >= 1e-2].astype(np.float32)
+    b = MeshBuilder()
+    b.add(kept.reshape(-1, 3), np.zeros((len(kept) * 3, 2), np.float32), np.arange(len(kept) * 3, dtype=np.uint32).reshape(-1, 3))
+    return scene_of([b.geometry()])
+
+
 _backend = None
 
 
-def device_builders_agree(scene, rays, hb):
-    """The emulated renderer over a device-built tree: closest hits == the host check's (already compared with brute
-    force); occlusion == the same kernel's answer over the host-built tree."""
-    want_any = None
+def device_builders_agree(scene, rays, hb, occ):
+    """The emulated renderer over each builder's tree: closest hits == the host check's (already compared with brute
+    force); occlusion == brute force's."""
     for builder in ("host", "device", "device_lbvh"):
         r = _backend.RenderCUDA(0, bvh_builder=builder)
         r.initialize(8, 8)
         r.set_scene(scene)
         if not np.array_equal(r.trace_closest(rays).view(np.uint32), hb.view(np.uint32)):
             return False
-        got_any = r.trace_any(rays)
-        if want_any is None:
-            want_any = got_any
-        elif not np.array_equal(got_any, want_any):
+        if not np.array_equal(r.trace_any(rays).astype(bool), occ):
             return False
     return True
 
 
-def one(seed, device=False):
+def one(seed, device=False, hostcheck=HostCheck):
+    """Seed ``seed`` against brute force; ``hostcheck(scene, threads)`` makes the host check that is compared."""
     rng = np.random.default_rng(seed)
     scene_scale = 10.0 ** rng.uniform(-3, 3)
     geoms = [random_geometry(rng, scene_scale) for _ in range(int(rng.integers(1, 4)))]
-    scene = Scene(meshes=[Mesh(geoms)], parameterized_meshes=[ParameterizedMesh(0, [0] * len(geoms))],
-                  instances=[Instance(np.eye(4, dtype=np.float32), 0)], materials=[DisneyMaterial()], textures=[],
-                  lights=[default_obj_light()], samples_per_pixel=1)
+    scene = scene_of(geoms)
     rays = random_rays(rng, scene, 600)
+    threads = int(rng.integers(0, 4))
+    # the comparison is about the hierarchy, not the formula: both sides run on the scene without its needles
+    scene = without_needles(scene)
+    if scene.total_tris() == 0:
+        return True, (True, True, True, 0)
     brute = OracleBackend(brute_force=True)
     brute.initialize(8, 8)
     brute.set_scene(scene)
-    hc = HostCheck(scene, int(rng.integers(0, 4)))
+    hc = hostcheck(scene, threads)
     hb, _, _ = hc.trace(rays)
     ho = brute.trace_closest(rays)
-    # Needle triangles are ill-conditioned for the triangle formula itself: the computed t can be off by far more
-    # than rounding (seed 98: a 0.04-long sliver 800 units away "hit" at t = 800.911 while its box spans
-    # [800.939, 800.943]), so no hierarchy can agree with brute force on them. Rays whose brute-force or product
-    # answer involves such a triangle are set aside; everything else must match bit for bit.
-    tris = np.concatenate([np.asarray(g.vertices, np.float32)[np.asarray(g.indices, np.uint32).reshape(-1, 3)]
-                           for g in scene.meshes[0].geometries]).astype(np.float64)
-    e = [tris[:, 1] - tris[:, 0], tris[:, 2] - tris[:, 0], tris[:, 2] - tris[:, 1]]
-    longest = np.maximum(np.maximum((e[0] ** 2).sum(1), (e[1] ** 2).sum(1)), (e[2] ** 2).sum(1))
-    quality = np.linalg.norm(np.cross(e[0], e[1]), axis=1) / np.maximum(longest, 1e-300)  # 2 * area / longest edge^2
-    needle = quality < 1e-2
-    if needle.any():
-        # re-run both on the scene without the needles: the comparison is about the hierarchy, not the formula
-        keep = ~needle
-        b = MeshBuilder()
-        kept = tris[keep].astype(np.float32)
-        if len(kept) == 0:
-            return True, (True, True, 0)
-        b.add(kept.reshape(-1, 3), np.zeros((len(kept) * 3, 2), np.float32), np.arange(len(kept) * 3, dtype=np.uint32).reshape(-1, 3))
-        scene = Scene(meshes=[Mesh([b.geometry()])], parameterized_meshes=[ParameterizedMesh(0, [0])],
-                      instances=[Instance(np.eye(4, dtype=np.float32), 0)], materials=[DisneyMaterial()], textures=[],
-                      lights=[default_obj_light()], samples_per_pixel=1)
-        brute = OracleBackend(brute_force=True)
-        brute.initialize(8, 8)
-        brute.set_scene(scene)
-        hc = HostCheck(scene, 0)
-        hb, _, _ = hc.trace(rays)
-        ho = brute.trace_closest(rays)
     same_closest = np.array_equal(hb.view(np.uint32), ho.view(np.uint32))
     ha, _, _ = hc.trace(rays, any_hit=True)
     hf, _, _ = hc.trace(rays, any_hit=True, far_first=True)
     occ = brute.trace_any(rays).astype(bool)
     same_any = np.array_equal(ha[:, 3].view(np.uint32) != 0xFFFFFFFF, occ) and np.array_equal(hf[:, 3].view(np.uint32) != 0xFFFFFFFF, occ)
     same_device = True
-    if device and scene.total_tris() > 0:
-        same_device = device_builders_agree(scene, rays, hb)
+    if device:
+        same_device = device_builders_agree(scene, rays, hb, occ)
     return same_closest and same_any and same_device, (same_closest, same_any, same_device, scene.total_tris())
 
 

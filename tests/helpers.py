@@ -84,12 +84,14 @@ def reference_result(golden_path, name, index, available, live, to_record=None):
 
 class HostCheck:
     """ctypes binding of the TEST-ONLY libcrt_bvh8_hostcheck.so (host instantiation of the
-    product's BVH8 builder + traversal)."""
+    product's BVH8 builder + traversal). ``variant``: "rcp_lo" / "rcp_hi" load the builds whose box-test reciprocal is
+    one ulp towards / away from zero (Makefile)."""
 
-    def __init__(self, scene, threads=0):
+    def __init__(self, scene, threads=0, variant=None):
         from chameleonrt_b200.scene import CScene
 
-        lib = C.CDLL(os.path.join(ROOT, "chameleonrt_b200", "csrc", "libcrt_bvh8_hostcheck.so"))
+        name = "libcrt_bvh8_hostcheck" + (f"_{variant}" if variant else "") + ".so"
+        lib = C.CDLL(os.path.join(ROOT, "chameleonrt_b200", "csrc", name))
         lib.crt_hostcheck_create.restype = C.c_void_p
         lib.crt_hostcheck_create.argtypes = [C.POINTER(CScene), C.c_int]
         lib.crt_hostcheck_destroy.argtypes = [C.c_void_p]

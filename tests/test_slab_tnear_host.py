@@ -2,7 +2,8 @@
 exact for tnear >= 0, which every ray of a frame has; caller-supplied rays (crtc_trace_closest) may start at a negative
 tnear, where the integer order of negative floats is reversed and the test must stay conservative. Rays whose origin
 has been moved past part of the scene, with tnear < 0 reaching back to the camera, must give the oracle's hits bit for
-bit. CPU only (the host instantiation of the traversal, libcrt_bvh8_hostcheck.so)."""
+bit. CPU only: this runs the single-ray host instantiation of the traversal (libcrt_bvh8_hostcheck.so), which checks the
+box test but not k_traverse's warp-pooled hit merge; tests/test_traversal_edges.py runs the kernel on such rays."""
 import numpy as np
 
 from chameleonrt_b200.scenes import sponza_like
