@@ -77,6 +77,11 @@ RenderCUDA::RenderCUDA(bool native_display_) : native_display(native_display_)
         throw std::runtime_error("crt_cuda: CRT_CUDA_DENOISE needs the whole frame on one GPU; it cannot be combined with "
                                  "more than one device in CRT_CUDA_DEVICES");
     }
+    // CRT_CUDA_DENOISE_HISTORY=H: the denoiser carries a reprojected history of up to H samples across camera moves
+    const int64_t denoise_history = env_or("CRT_CUDA_DENOISE_HISTORY", 0);
+    if (denoise_history != 0 && !denoise) {
+        throw std::runtime_error("crt_cuda: CRT_CUDA_DENOISE_HISTORY is the denoiser's history; it needs CRT_CUDA_DENOISE=1");
+    }
     try {
         for (size_t i = 0; i < devices.size(); ++i) {
             crtc_renderer *r = nullptr;
@@ -92,6 +97,9 @@ RenderCUDA::RenderCUDA(bool native_display_) : native_display(native_display_)
             check(crtc_set_option(r, "hw_textures", env_or("CRT_CUDA_HW_TEXTURES", 0)));  // 1 = texels through cudaTextureObject_t (crt_cuda.h)
             check(crtc_set_option(r, "stage_events", env_or("CRT_CUDA_STAGE_EVENTS", 1)));  // 0 = no per-stage timings (crt_cuda_get_stats reads 0)
             check(crtc_set_option(r, "aov", denoise ? 1 : 0));  // CRT_CUDA_DENOISE: first-hit AOVs for crtc_denoise
+            if (denoise_history != 0) {
+                check(crtc_set_option(r, "denoise_history", denoise_history));  // (out of range: refused here)
+            }
         }
     } catch (...) {
         for (crtc_renderer *r : renderers) {

@@ -36,11 +36,14 @@ C_ABI_SYMBOLS = (
     "crtc_initialize", "crtc_set_scene", "crtc_render", "crtc_render_async", "crtc_sync", "crtc_read_accum", "crtc_get_stage_times",
     "crtc_get_counters", "crtc_get_scene_info", "crtc_trace_closest", "crtc_trace_any", "crtc_bench_trace",
     "crtc_local_buffers", "crtc_assemble_rank", "crtc_export_frame", "crtc_import_frame", "crtc_share_frame", "crtc_read_img", "crtc_frame_wait", "crtc_copy_img_to_array",
-    "crtc_read_aov", "crtc_denoise",
+    "crtc_read_aov", "crtc_denoise", "crtc_read_denoise_history",
 )
 # Per-pixel layout of crtc_read_aov: name -> (first float, number of floats)
 AOV_LAYOUT = {"albedo": (0, 3), "coverage": (3, 1), "normal": (4, 3), "depth": (7, 1), "lum_m1": (8, 1), "lum_m2": (9, 1)}
 AOV_FLOATS = 10
+# Per-pixel layout of crtc_read_denoise_history
+HISTORY_LAYOUT = {"color": (0, 3), "lum_m1": (3, 1), "lum_m2": (4, 1), "count": (5, 1), "depth": (6, 1), "normal": (7, 3)}
+HISTORY_FLOATS = 10
 
 
 class CDenoiseParams(C.Structure):
@@ -94,6 +97,7 @@ def load_lib() -> C.CDLL:
     lib.crtc_share_frame.argtypes = [vp, vp]
     lib.crtc_read_aov.argtypes = [vp, vp]
     lib.crtc_denoise.argtypes = [vp, C.POINTER(CDenoiseParams), vp, vp, vp]
+    lib.crtc_read_denoise_history.argtypes = [vp, vp]
     _lib = lib
     return lib
 
@@ -109,7 +113,8 @@ class RenderCUDA:
     def __init__(self, device: int = 0, max_depth: int = 5, rank: int = 0, world_size: int = 1,
                  count_traversal: bool = False, bvh_threads: int = 0, stream: Optional[int] = None,
                  any_far_first: Optional[int] = None, bvh_builder: Optional[str] = None,
-                 tri_pass_defer: Optional[int] = None, shade_sort: Optional[int] = None, aov: bool = False):
+                 tri_pass_defer: Optional[int] = None, shade_sort: Optional[int] = None, aov: bool = False,
+                 denoise_history: int = 0):
         self.lib = load_lib()
         self.h = C.c_void_p()
         self._check(self.lib.crtc_create(C.byref(self.h), device))
@@ -147,6 +152,8 @@ class RenderCUDA:
             self._check(self.lib.crtc_set_option(self.h, b"bvh_builder", names.index(bvh_builder)))
         if aov:  # first-hit AOVs with every frame, for read_aov() and denoise() (crt_cuda.h: option "aov")
             self._check(self.lib.crtc_set_option(self.h, b"aov", 1))
+        if denoise_history:  # denoise() carries a reprojected history of up to this many samples (option "denoise_history")
+            self._check(self.lib.crtc_set_option(self.h, b"denoise_history", int(denoise_history)))
         if stream is not None:
             self._check(self.lib.crtc_set_stream(self.h, C.c_void_p(stream)))
         self.width = self.height = 0
@@ -264,6 +271,14 @@ class RenderCUDA:
         img = np.zeros((self.height, self.width), dtype=np.uint32)
         self._check(self.lib.crtc_denoise(self.h, C.byref(prm), rgb.ctypes.data, img.ctypes.data, None))
         return rgb, img
+
+    def read_denoise_history(self) -> dict:
+        """The history the last denoise() wrote (crtc_read_denoise_history; needs ``denoise_history`` > 0): ``color``
+        (h, w, 3, integrated demodulated colour), ``lum_m1`` / ``lum_m2`` (h, w, integrated luminance moments), ``count``
+        (h, w, the samples they represent), ``depth`` (h, w) and ``normal`` (h, w, 3, unit), all float32."""
+        a = np.zeros((self.height, self.width, HISTORY_FLOATS), dtype=np.float32)
+        self._check(self.lib.crtc_read_denoise_history(self.h, a.ctypes.data))
+        return {k: (a[:, :, o:o + n] if n > 1 else a[:, :, o]).copy() for k, (o, n) in HISTORY_LAYOUT.items()}
 
     def stage_times(self) -> dict:
         a = np.zeros(len(STAGE_NAMES), dtype=np.float32)

@@ -260,20 +260,196 @@ __global__ void __launch_bounds__(kDenoiseBlock) k_dn_atrous(int w, int h, int s
     img_out[p] = float_to_srgb8(rgb.x) | (float_to_srgb8(rgb.y) << 8) | (float_to_srgb8(rgb.z) << 16) | 0xff000000u;
 }
 
+// ---- the denoiser's temporal history (option "denoise_history"; include/crt_cuda.h, crtc_denoise) ----
+// Per framebuffer pixel, kHistFloats floats: integrated demodulated colour I.rgb, integrated luminance moments M1 and M2,
+// the number of samples n they represent, the first-hit depth z and unit normal of the frame they were written for.
+constexpr int kHistFloats = 10;
+constexpr int kHistColor = 0, kHistM1 = 3, kHistM2 = 4, kHistCount = 5, kHistDepth = 6, kHistNormal = 7;
+
+// The camera a history was written for: its position and the inverse of the matrix [du | dv | tl] (row-major; inverted
+// in double on the host, rounded to float)
+struct HistoryView {
+    float3 pos;
+    float minv[9];
+};
+
+// One thread per pixel, after k_dn_prepare. Reprojects the pixel's first hit into the previous camera, blends the
+// valid bilinear taps of `prev` (null: no history) with this epoch's accum and moments, writes the result to `cur` and
+// the blended colour to iv.xyz. Pixels without history keep k_dn_prepare's iv bits.
+__global__ void __launch_bounds__(kDenoiseBlock) k_dn_temporal(int w, int h, float samples, float max_history, ViewParams view,
+                                                               HistoryView pv, const float *prev, const float *aov,
+                                                               const float4 *guide, float4 *iv, float *cur)
+{
+    const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= (uint32_t)w * (uint32_t)h) {
+        return;
+    }
+    const int x = (int)(p % (uint32_t)w), y = (int)(p / (uint32_t)w);
+    const float *a = aov + (size_t)kAovFloats * p;
+    const float4 gp = guide[p];
+    const float3 np = mk3(gp.x, gp.y, gp.z);
+    float n_p = 0.f;
+    float hist[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
+    if (prev && a[kAovCoverage] > 0.f) {
+        // the world point of the pixel-centre ray (k_raygen's expression, jitter 0.5) at the AOV depth
+        const float px_x = ((float)x + 0.5f) / (float)(uint32_t)w;
+        const float px_y = ((float)y + 0.5f) / (float)(uint32_t)h;
+        const float3 d = normalize(mk3(view.dir_du.x * px_x + view.dir_dv.x * px_y + view.dir_top_left.x,
+                                       view.dir_du.y * px_x + view.dir_dv.y * px_y + view.dir_top_left.y,
+                                       view.dir_du.z * px_x + view.dir_dv.z * px_y + view.dir_top_left.z));
+        const float3 r = mk3(view.pos.x + gp.w * d.x, view.pos.y + gp.w * d.y, view.pos.z + gp.w * d.z) - pv.pos;
+        const float al = pv.minv[0] * r.x + pv.minv[1] * r.y + pv.minv[2] * r.z;
+        const float be = pv.minv[3] * r.x + pv.minv[4] * r.y + pv.minv[5] * r.z;
+        const float ga = pv.minv[6] * r.x + pv.minv[7] * r.y + pv.minv[8] * r.z;
+        const float sx = (al / ga) * (float)w - 0.5f, sy = (be / ga) * (float)h - 0.5f;
+        // (outside this window every tap is outside the image; it also keeps NaN and huge values away from the int cast)
+        if (ga > 0.f && sx > -1.f && sx < (float)w && sy > -1.f && sy < (float)h) {
+            const float dist = length(r);
+            const float fx0 = floorf(sx), fy0 = floorf(sy);
+            const float fx = sx - fx0, fy = sy - fy0;
+            const int x0 = (int)fx0, y0 = (int)fy0;
+            float sw = 0.f, sn = 0.f;
+            float acc[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+            for (int t = 0; t < 4; ++t) {
+                const int qx = x0 + (t & 1), qy = y0 + (t >> 1);
+                if (qx < 0 || qx >= w || qy < 0 || qy >= h) {
+                    continue;
+                }
+                const float *hq = prev + (size_t)kHistFloats * ((size_t)qy * w + qx);
+                const float3 nq = mk3(hq[kHistNormal], hq[kHistNormal + 1], hq[kHistNormal + 2]);
+                if (all_zero(nq)) {
+                    continue;
+                }
+                // prev's depth gradient at q, as k_dn_prepare computes it
+                const int xl = qx > 0 ? qx - 1 : qx, xr = qx < w - 1 ? qx + 1 : qx, yu = qy > 0 ? qy - 1 : qy,
+                          yd = qy < h - 1 ? qy + 1 : qy;
+                const float zx = prev[(size_t)kHistFloats * ((size_t)qy * w + xr) + kHistDepth] -
+                                 prev[(size_t)kHistFloats * ((size_t)qy * w + xl) + kHistDepth];
+                const float zy = prev[(size_t)kHistFloats * ((size_t)yd * w + qx) + kHistDepth] -
+                                 prev[(size_t)kHistFloats * ((size_t)yu * w + qx) + kHistDepth];
+                const float gx = xr - xl == 2 ? 0.5f * zx : zx, gy = yd - yu == 2 ? 0.5f * zy : zy;
+                if (!(fabsf(hq[kHistDepth] - dist) <= 0.02f * dist + 2.f * (fabsf(gx) + fabsf(gy))) || !(dot(np, nq) >= 0.9f)) {
+                    continue;
+                }
+                const float wt = ((t & 1) ? fx : 1.f - fx) * ((t >> 1) ? fy : 1.f - fy);
+                sw += wt;
+                sn += wt * hq[kHistCount];
+#pragma unroll
+                for (int j = 0; j < 5; ++j) {
+                    acc[j] += wt * hq[j];
+                }
+            }
+            if (sw >= 0.01f) {
+#pragma unroll
+                for (int j = 0; j < 5; ++j) {
+                    hist[j] = acc[j] / sw;
+                }
+                n_p = fminf(max_history, sn / sw);
+            }
+        }
+    }
+    const float4 c = iv[p];
+    float now[5] = {c.x, c.y, c.z, a[kAovLumM1], a[kAovLumM2]};
+    float n_t = samples;
+    if (n_p > 0.f) {
+        n_t = n_p + samples;
+#pragma unroll
+        for (int j = 0; j < 5; ++j) {
+            now[j] = (n_p * hist[j] + samples * now[j]) / n_t;
+        }
+        iv[p] = make_float4(now[0], now[1], now[2], c.w);
+    }
+    float *o = cur + (size_t)kHistFloats * p;
+#pragma unroll
+    for (int j = 0; j < 5; ++j) {
+        o[j] = now[j];
+    }
+    o[kHistCount] = n_t;
+    o[kHistDepth] = gp.w;
+    o[kHistNormal] = gp.x;
+    o[kHistNormal + 1] = gp.y;
+    o[kHistNormal + 2] = gp.z;
+}
+
+// One thread per pixel, after k_dn_temporal: iv.w = max(0, M2 - M1^2) / n from the integrated moments where n >= 4;
+// where n < 4, from moments averaged over the 7x7 neighbourhood with the a-trous's normal and depth weights at step 1
+// (taps outside the image skipped; no luminance or kernel weight).
+__global__ void __launch_bounds__(kDenoiseBlock) k_dn_variance(int w, int h, float sigma_n, float sigma_z, const float *cur,
+                                                               const float4 *guide, const float2 *grad, float4 *iv)
+{
+    const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= (uint32_t)w * (uint32_t)h) {
+        return;
+    }
+    const int x = (int)(p % (uint32_t)w), y = (int)(p / (uint32_t)w);
+    const float *hp = cur + (size_t)kHistFloats * p;
+    const float n_t = hp[kHistCount];
+    float m1 = hp[kHistM1], m2 = hp[kHistM2];
+    if (n_t < 4.f) {
+        const float4 gp = guide[p];
+        const float2 dz = grad[p];
+        const bool p_bg = gp.x == 0.f && gp.y == 0.f && gp.z == 0.f;
+        float sw = 0.f, s1 = 0.f, s2 = 0.f;
+        for (int dy = -3; dy <= 3; ++dy) {
+            for (int dx = -3; dx <= 3; ++dx) {
+                const int qx = x + dx, qy = y + dy;
+                if (qx < 0 || qx >= w || qy < 0 || qy >= h) {
+                    continue;
+                }
+                const size_t q = (size_t)qy * w + qx;
+                const float4 gq = guide[q];
+                const bool q_bg = gq.x == 0.f && gq.y == 0.f && gq.z == 0.f;
+                float w_n;
+                if (p_bg || q_bg) {
+                    w_n = p_bg && q_bg ? 1.f : 0.f;
+                } else {
+                    w_n = powf(fmaxf(0.f, gp.x * gq.x + gp.y * gq.y + gp.z * gq.z), sigma_n);
+                }
+                const float w_z = expf(-fabsf(gp.w - gq.w) / (sigma_z * fabsf(dz.x * (float)dx + dz.y * (float)dy) + 1e-3f));
+                const float wt = w_n * w_z;
+                sw += wt;
+                s1 += wt * cur[(size_t)kHistFloats * q + kHistM1];
+                s2 += wt * cur[(size_t)kHistFloats * q + kHistM2];
+            }
+        }
+        m1 = s1 / sw;
+        m2 = s2 / sw;
+    }
+    const float4 c = iv[p];
+    iv[p] = make_float4(c.x, c.y, c.z, fmaxf(0.f, m2 - m1 * m1) / n_t);
+}
+
 struct DenoiseParams {
     int iterations = 5;
     float sigma_l = 4.f, sigma_n = 128.f, sigma_z = 1.f;
 };
 
+// What a history buffer was written for: the reset epoch and the camera of that epoch's first frame
+struct HistoryTag {
+    bool valid = false;
+    uint64_t epoch = 0;
+    ViewParams view{};
+};
+
 // The renderer's AOV and denoiser state. AOV buffers: 40 B per local pixel (tile-padded) + 40 B per framebuffer pixel;
-// denoiser buffers, allocated by the first denoise call: 72 B per framebuffer pixel.
+// denoiser buffers, allocated by the first denoise call: 72 B per framebuffer pixel, + 80 B with option denoise_history
+// (the two history buffers, `prev` and `cur`).
 struct AovState {
     crt_host::DeviceBuffer<float> local, full;
     crt_host::DeviceBuffer<float4> dn_iv[2], dn_guide;
     crt_host::DeviceBuffer<float2> dn_grad;
     crt_host::DeviceBuffer<float> dn_rgb;
     crt_host::DeviceBuffer<uint32_t> dn_img;
+    crt_host::DeviceBuffer<float> hist[2];  // hist[hist_cur] is `cur`, the other one `prev`
+    HistoryTag hist_tag[2];
+    int hist_cur = 0;
 
+    void drop_history()
+    {
+        hist_tag[0] = HistoryTag{};
+        hist_tag[1] = HistoryTag{};
+    }
     void release()
     {
         local.release();
@@ -284,6 +460,41 @@ struct AovState {
         dn_grad.release();
         dn_rgb.release();
         dn_img.release();
+        hist[0].release();
+        hist[1].release();
+        drop_history();
+    }
+    // `cur` if the last denoise call was made in `epoch`, else null
+    const float *history_of(uint64_t epoch) const
+    {
+        const HistoryTag &t = hist_tag[hist_cur];
+        return t.valid && t.epoch == epoch ? hist[hist_cur].ptr : nullptr;
+    }
+    // The previous camera for k_dn_temporal: false if [du | dv | tl] is singular or not finite (no reprojection then)
+    static bool history_view(const ViewParams &v, HistoryView &out)
+    {
+        const double m[3][3] = {{v.dir_du.x, v.dir_dv.x, v.dir_top_left.x},
+                                {v.dir_du.y, v.dir_dv.y, v.dir_top_left.y},
+                                {v.dir_du.z, v.dir_dv.z, v.dir_top_left.z}};
+        const double det = m[0][0] * (m[1][1] * m[2][2] - m[1][2] * m[2][1]) - m[0][1] * (m[1][0] * m[2][2] - m[1][2] * m[2][0]) +
+                           m[0][2] * (m[1][0] * m[2][1] - m[1][1] * m[2][0]);
+        if (!std::isfinite(det) || det == 0.0) {
+            return false;
+        }
+        // the adjugate over the determinant, row-major
+        const double inv[9] = {(m[1][1] * m[2][2] - m[1][2] * m[2][1]) / det, (m[0][2] * m[2][1] - m[0][1] * m[2][2]) / det,
+                               (m[0][1] * m[1][2] - m[0][2] * m[1][1]) / det, (m[1][2] * m[2][0] - m[1][0] * m[2][2]) / det,
+                               (m[0][0] * m[2][2] - m[0][2] * m[2][0]) / det, (m[0][2] * m[1][0] - m[0][0] * m[1][2]) / det,
+                               (m[1][0] * m[2][1] - m[1][1] * m[2][0]) / det, (m[0][1] * m[2][0] - m[0][0] * m[2][1]) / det,
+                               (m[0][0] * m[1][1] - m[0][1] * m[1][0]) / det};
+        for (int i = 0; i < 9; ++i) {
+            if (!std::isfinite(inv[i])) {
+                return false;
+            }
+            out.minv[i] = (float)inv[i];
+        }
+        out.pos = v.pos;
+        return true;
     }
     // (crtc_initialize) zeroed buffers for a new framebuffer; the denoiser's are reallocated on first use
     void allocate(size_t npx_local, size_t npx_full, cudaStream_t stream)
@@ -311,10 +522,14 @@ struct AovState {
         aov_launch(k_aov_moments, (f.npx_local + 255) / 256, 256, stream, f, ps, frame_id, local.ptr, full.ptr);
     }
     // Denoises the full frame `accum` (w x h x 3, `samples` = spp * frames accumulated) into dn_rgb / dn_img.
-    void denoise(int w, int h, float samples, const float *accum, const DenoiseParams &prm, cudaStream_t stream)
+    // max_history > 0 (option denoise_history): the temporal pass runs between k_dn_prepare and the a-trous chain, with
+    // the history of the latest earlier epoch that had a denoise call as `prev`; `epoch` and `view` are the current
+    // reset epoch and the camera of its first frame.
+    void denoise(int w, int h, float samples, const float *accum, const DenoiseParams &prm, uint32_t max_history,
+                 uint64_t epoch, const ViewParams &view, cudaStream_t stream)
     {
         const size_t n = (size_t)w * h;
-        if (dn_img.count != n) {
+        if (dn_img.count != n || (max_history && hist[0].count != kHistFloats * n)) {
             CUDA_CHECK(cudaStreamSynchronize(stream));
             dn_iv[0].alloc(n);
             dn_iv[1].alloc(n);
@@ -322,10 +537,31 @@ struct AovState {
             dn_grad.alloc(n);
             dn_rgb.alloc(3 * n);
             dn_img.alloc(n);
+            if (max_history) {
+                hist[0].alloc(kHistFloats * n);
+                hist[1].alloc(kHistFloats * n);
+                drop_history();
+            }
         }
         const unsigned g = (unsigned)((n + kDenoiseBlock - 1) / kDenoiseBlock);
         aov_launch(k_dn_prepare, g, kDenoiseBlock, stream, w, h, samples, accum, (const float *)full.ptr, dn_iv[0].ptr,
                    dn_guide.ptr, dn_grad.ptr);
+        if (max_history) {
+            if (hist_tag[hist_cur].valid && hist_tag[hist_cur].epoch < epoch) {
+                hist_cur ^= 1;  // cur -> prev; the older prev is overwritten
+            }
+            const HistoryTag &pt = hist_tag[hist_cur ^ 1];
+            HistoryView pv{};
+            const bool have_prev = pt.valid && pt.epoch < epoch && history_view(pt.view, pv);
+            aov_launch(k_dn_temporal, g, kDenoiseBlock, stream, w, h, samples, (float)max_history, view, pv,
+                       have_prev ? (const float *)hist[hist_cur ^ 1].ptr : nullptr, (const float *)full.ptr,
+                       (const float4 *)dn_guide.ptr, dn_iv[0].ptr, hist[hist_cur].ptr);
+            aov_launch(k_dn_variance, g, kDenoiseBlock, stream, w, h, prm.sigma_n, prm.sigma_z, (const float *)hist[hist_cur].ptr,
+                       (const float4 *)dn_guide.ptr, (const float2 *)dn_grad.ptr, dn_iv[0].ptr);
+            hist_tag[hist_cur].valid = true;
+            hist_tag[hist_cur].epoch = epoch;
+            hist_tag[hist_cur].view = view;
+        }
         for (int i = 0; i < prm.iterations; ++i) {
             const float4 *in = dn_iv[i & 1].ptr;
             float4 *out = dn_iv[(i + 1) & 1].ptr;

@@ -230,6 +230,12 @@ struct crtc_renderer {
     // option, `aov_active` what the last crtc_initialize set up.
     bool aov = false, aov_active = false;
     crt::AovState aov_state;
+    // option "denoise_history": the most samples crtc_denoise's temporal history may carry (0 = off); `dn_history_active`
+    // is what the last crtc_initialize set up. `epoch` counts accumulation resets that were followed by a frame;
+    // `epoch_view` is the camera of the current epoch's first frame.
+    uint32_t dn_history = 0, dn_history_active = 0;
+    uint64_t epoch = 0;
+    crt::ViewParams epoch_view{};
     void require_unshared_aov(const char *what) const
     {
         if (aov_active) {
@@ -605,6 +611,10 @@ struct crtc_renderer {
             throw std::runtime_error("initialize: option aov needs the whole frame on one renderer (world_size 1); "
                                      "AOVs of multi-GPU frames are not supported");
         }
+        if (dn_history && !aov) {
+            throw std::runtime_error("initialize: option denoise_history needs option aov = 1 (the history is built from the "
+                                     "first-hit AOVs)");
+        }
         make_current();
         CUDA_CHECK(cudaStreamSynchronize(stream));
         unpin_img();             // (the caller's img buffer is reallocated with the new size)
@@ -629,7 +639,8 @@ struct crtc_renderer {
         CUDA_CHECK(cudaMemsetAsync(d_accum_full.ptr, 0, (size_t)w * h * 3 * sizeof(float), stream));
         CUDA_CHECK(cudaMemsetAsync(d_img_full.ptr, 0, ((size_t)w * h + crt::kSyncWords) * 4, stream));
         aov_active = aov;
-        if (aov_active) {
+        dn_history_active = dn_history;
+        if (aov_active) {  // (drops the denoiser's history too)
             aov_state.allocate(npx_local, (size_t)w * h, stream);
         } else {
             aov_state.release();
@@ -732,6 +743,7 @@ struct crtc_renderer {
                 CUDA_CHECK(cudaMemsetAsync(aov_state.local.ptr, 0, (size_t)npx_local * crt::kAovFloats * sizeof(float), stream));
             }
         }
+        aov_state.drop_history();  // (a history of another scene does not reproject)
     }
 
     // Enqueues one frame on the stream (no host synchronisation) and returns its record.
@@ -754,6 +766,10 @@ struct crtc_renderer {
             frame_id = 0;  // render_embree.cpp:145-147
         }
         const crt::ViewParams view = crt::make_view_params(pos, dir, up, fovy, fb_w, fb_h, frame_id);
+        if (frame_id == 0) {  // the first frame since a reset starts a new epoch (crtc_denoise's history)
+            ++epoch;
+            epoch_view = view;
+        }
         const size_t npaths = (size_t)npx_local * spp * num_frames;
         if (npaths >= 0x7fffffffull) {
             throw std::runtime_error("render: more than 2^31 paths in flight on one device");
@@ -1137,6 +1153,22 @@ struct crtc_renderer {
         CUDA_CHECK(cudaGetLastError());
     }
 
+    void read_denoise_history(float *out)
+    {
+        if (!dn_history_active) {
+            throw std::runtime_error("crtc_read_denoise_history: option denoise_history is off (set it before crtc_initialize)");
+        }
+        const float *cur = aov_state.history_of(epoch);
+        if (!cur || frame_id == 0) {
+            throw std::runtime_error("crtc_read_denoise_history: no crtc_denoise since the last reset");
+        }
+        make_current();
+        CUDA_CHECK(cudaMemcpyAsync(out, cur, (size_t)fb_w * fb_h * crt::kHistFloats * sizeof(float), cudaMemcpyDeviceToHost,
+                                   stream));
+        CUDA_CHECK(cudaStreamSynchronize(stream));
+        CUDA_CHECK(cudaGetLastError());
+    }
+
     void denoise(const crtc_denoise_params_t *params, float *rgb_out, uint32_t *img_out, void *cuda_array)
     {
         crt::DenoiseParams p;
@@ -1157,7 +1189,8 @@ struct crtc_renderer {
         }
         require_aov_frame("crtc_denoise");
         make_current();
-        aov_state.denoise(fb_w, fb_h, (float)spp * (float)frame_id, d_accum_full.ptr, p, stream);
+        aov_state.denoise(fb_w, fb_h, (float)spp * (float)frame_id, d_accum_full.ptr, p, dn_history_active, epoch, epoch_view,
+                          stream);
         const size_t n = (size_t)fb_w * fb_h;
         if (rgb_out) {
             CUDA_CHECK(cudaMemcpyAsync(rgb_out, aov_state.dn_rgb.ptr, n * 3 * sizeof(float), cudaMemcpyDeviceToHost, stream));
@@ -1332,6 +1365,11 @@ int crtc_set_option(crtc_renderer *r, const char *key, int64_t value)
             r->count_traversal = value != 0;
         } else if (k == "aov") {
             r->aov = value != 0;  // takes effect at the next crtc_initialize
+        } else if (k == "denoise_history") {
+            if (value < 0 || value > 1024) {
+                throw std::runtime_error("denoise_history must be in [0, 1024] (0 = off)");
+            }
+            r->dn_history = (uint32_t)value;  // takes effect at the next crtc_initialize
         } else if (k == "refill_idle") {
             r->refill_idle = (int)std::min<int64_t>(std::max<int64_t>(value, 1), 32);
         } else if (k == "any_far_first") {
@@ -1379,6 +1417,8 @@ int crtc_get_option(crtc_renderer *r, const char *key, int64_t *value)
             *value = r->count_traversal ? 1 : 0;
         } else if (k == "aov") {
             *value = r->aov ? 1 : 0;
+        } else if (k == "denoise_history") {
+            *value = r->dn_history;
         } else if (k == "refill_idle") {
             *value = r->refill_idle;
         } else if (k == "any_far_first") {
@@ -1480,6 +1520,16 @@ int crtc_read_aov(crtc_renderer *r, float *out)
 int crtc_denoise(crtc_renderer *r, const crtc_denoise_params_t *params, float *rgb_out, uint32_t *img_out, void *cuda_array)
 {
     CRTC_TRY({ require_renderer(r); r->denoise(params, rgb_out, img_out, cuda_array); })
+}
+
+int crtc_read_denoise_history(crtc_renderer *r, float *out)
+{
+    CRTC_TRY({ require_renderer(r);
+        if (!out) {
+            throw std::runtime_error("crtc_read_denoise_history: out is NULL");
+        }
+        r->read_denoise_history(out);
+    })
 }
 
 int crtc_get_stage_times(crtc_renderer *r, float *ms_out, int n)

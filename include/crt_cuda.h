@@ -110,6 +110,12 @@ void crtc_destroy(crtc_renderer *r);
  *                 state and write only their own buffers: accum, img and the ray counts are the same with the option on.
  *                 Memory: 40 B per pixel of the local tiles (64x64-padded) + 40 B per framebuffer pixel; the first
  *                 crtc_denoise adds 72 B per framebuffer pixel (1920x1080: 166 MB of AOVs + 149 MB for the denoiser).
+ *   "denoise_history" H in 0..1024, 0 (default) = off: crtc_denoise carries a temporal history across accumulation
+ *                 resets (camera moves), reprojected into the current camera and capped at H samples (see crtc_denoise).
+ *                 Takes effect at the next crtc_initialize, which fails if it is nonzero with option aov = 0; out of
+ *                 range is an error. Nothing runs in the frame path: two more kernels run inside crtc_denoise only. Memory:
+ *                 the first crtc_denoise adds 80 B per framebuffer pixel (two history buffers of 10 floats; 1920x1080:
+ *                 166 MB). crtc_initialize and crtc_set_scene drop the history.
  */
 int crtc_set_option(crtc_renderer *r, const char *key, int64_t value);
 
@@ -246,8 +252,8 @@ typedef struct crtc_denoise_params_t {
     float sigma_depth;     /* default 1:   w_z = exp(-|Z_p - Z_q| / (sigma_depth * |grad Z_p . step offset| + 1e-3)) */
 } crtc_denoise_params_t;
 
-/* Edge-aware a-trous denoiser over the accumulated frame (the spatial part of SVGF, Schied et al. 2017; no temporal
- * reprojection: accumulation covers a still camera). Needs option "aov" and a frame, like crtc_read_aov.
+/* Edge-aware a-trous denoiser over the accumulated frame (the spatial part of SVGF, Schied et al. 2017; the temporal part,
+ * below, only with option "denoise_history"). Needs option "aov" and a frame, like crtc_read_aov.
  *   1. I = accum / max(albedo, 1e-3) per channel; v = max(0, lum_m2 - lum_m1^2) / (spp * frames accumulated).
  *   2. K iterations i = 0..K-1 with step h = 2^i over a 5x5 B3-spline kernel (1,4,6,4,1)/16 per axis, taps outside the
  *      image skipped, dy outer and dx inner. Per tap q of pixel p: w = k * w_l * w_n * w_z, where the luminance weight
@@ -259,8 +265,37 @@ typedef struct crtc_denoise_params_t {
  * params: NULL = the defaults; out of range (iterations outside 1..10, a sigma not finite or <= 0) is an error.
  * Outputs, each optional: rgb_out (HOST, fb_width*fb_height*3 floats), img_out (HOST, fb_width*fb_height RGBA8),
  * cuda_array (a cudaArray_t, as crtc_copy_img_to_array). All work runs on the renderer's stream (crtc_set_stream); returns
- * when the outputs are written. Scratch buffers (72 B per pixel) are allocated by the first call after crtc_initialize. */
+ * when the outputs are written. Scratch buffers (72 B per pixel) are allocated by the first call after crtc_initialize.
+ *
+ * Temporal history (option "denoise_history" = H > 0; SVGF's temporal half over a static scene). An epoch is the run of
+ * frames since an accumulation reset (crtc_initialize, crtc_set_scene, a render with camera_changed); the renderer keeps
+ * the camera of each epoch's first frame. Two history buffers of 10 floats per pixel, `prev` and `cur`, hold
+ * (I.rgb, M1, M2, n, z, nhat.xyz): integrated demodulated colour, integrated luminance moments, the samples they
+ * represent, and the depth and unit normal of step 1. A call in epoch e first turns `cur` into `prev` if `cur` was written
+ * in an earlier epoch, so `prev` is the output of the last call of the latest earlier epoch that had one; every call
+ * overwrites `cur`. crtc_initialize and crtc_set_scene drop both. Between steps 1 and 2 above, per pixel p = (x, y):
+ *   a. N = spp * frames accumulated (as in step 1). n_p = 0 if there is no `prev` or p's coverage is 0. Otherwise:
+ *   b. d = normalize(du * ((x + 0.5) / w) + dv * ((y + 0.5) / h) + tl) with the current camera's basis (the primary ray
+ *      expression at jitter 0.5), X = pos + z * d, z = p's AOV depth.
+ *   c. (alpha, beta, gamma) = M'^-1 (X - pos') with M' = [du' | dv' | tl'] of prev's camera (inverted in double, rounded to
+ *      float). Needs gamma > 0; then sx = (alpha / gamma) * w - 0.5, sy = (beta / gamma) * h - 0.5 and the 2x2 taps q
+ *      around (sx, sy) get bilinear weights. A tap is valid when it is inside the image, prev's normal at q is nonzero,
+ *      |z_q - |X - pos'|| <= 0.02 |X - pos'| + 2 (|gx_q| + |gy_q|) (g = prev's depth gradient at q, as in step 2) and
+ *      dot(nhat_p, nhat_q) >= 0.9. W = the sum of the valid taps' weights; if W < 0.01, n_p = 0, else
+ *      P = sum w prev_q / W for I.rgb, M1, M2 and n_p = min(H, sum w n_q / W).
+ *   d. n_t = n_p + N; I_t = (n_p P_I + N I) / n_t with I of step 1, and the same for M1, M2 with lum_m1, lum_m2. Where
+ *      n_p = 0 nothing is blended: I_t = I, M_t = lum_m, n_t = N. cur = (I_t, M1_t, M2_t, n_t, z, nhat); I = I_t.
+ *   e. v = max(0, M2_t - M1_t^2) / n_t where n_t >= 4. Where n_t < 4, M1_t and M2_t are first replaced by their mean over
+ *      the 7x7 neighbourhood (taps outside the image skipped) weighted by w_n * w_z of step 2 at h = 1 (this call's
+ *      sigma_normal, sigma_depth; no luminance or kernel weight): a 1-spp frame gets a nonzero variance.
+ * The history holds the integrated colour before filtering, so with a still camera its weight n_p / (n_p + N) falls as
+ * frames accumulate and the output converges to the history-off result. Without history in a pixel and with N >= 4, the
+ * output is bit-identical to the history-off denoiser's. */
 int crtc_denoise(crtc_renderer *r, const crtc_denoise_params_t *params, float *rgb_out, uint32_t *img_out, void *cuda_array);
+
+/* Option "denoise_history": `cur`, fb_width*fb_height*10 floats, row-major (I.rgb, M1, M2, n, z, nhat.xyz per pixel, as
+ * in crtc_denoise). Fails if the option is off or no crtc_denoise has run since the last reset. */
+int crtc_read_denoise_history(crtc_renderer *r, float *out);
 
 #ifdef __cplusplus
 }

@@ -75,7 +75,17 @@ def main():
     del renderers
 
     denoise_ms = {}
+    history_ms = {}
     prm = CDenoiseParams(5, 4.0, 128.0, 1.0)
+
+    def timed(r, stream):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        r._check(r.lib.crtc_denoise(r.h, C.byref(prm), None, None, None))
+        e1.record(stream)
+        e1.synchronize()
+        return e0.elapsed_time(e1)
+
     for w, h in ((1280, 720), (1920, 1080)):
         stream = torch.cuda.Stream()
         r = RenderCUDA(0, max_depth=8, aov=True, stream=stream.cuda_stream)
@@ -84,16 +94,25 @@ def main():
         r.render(*view, True, True)
         for _ in range(3):
             r._check(r.lib.crtc_denoise(r.h, C.byref(prm), None, None, None))
-        times = []
-        for _ in range(args.denoise_iters):
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record(stream)
-            r._check(r.lib.crtc_denoise(r.h, C.byref(prm), None, None, None))
-            e1.record(stream)
-            e1.synchronize()
-            times.append(e0.elapsed_time(e1))
+        times = [timed(r, stream) for _ in range(args.denoise_iters)]
         denoise_ms[(w, h)] = (float(np.median(times)), float(np.min(times)))
-        del r
+        # denoise_history = 32 after a camera move (a history to reproject), alternated call by call with a history-off
+        # renderer on the same stream and frame
+        rh = RenderCUDA(0, max_depth=8, aov=True, denoise_history=32, stream=stream.cuda_stream)
+        rh.initialize(w, h)
+        rh.set_scene(scene)
+        rh.render(*view, True, True)
+        rh._check(rh.lib.crtc_denoise(rh.h, C.byref(prm), None, None, None))
+        moved = ArcballCamera(tuple(np.asarray(cam["eye"]) + np.array([0.05, 0.0, 0.0])), cam["center"], cam["up"])
+        rh.render(moved.eye(), moved.dir(), moved.up(), cam["fov_y"], True, True)
+        for _ in range(3):
+            rh._check(rh.lib.crtc_denoise(rh.h, C.byref(prm), None, None, None))
+        on, off = [], []
+        for _ in range(args.denoise_iters):
+            on.append(timed(rh, stream))
+            off.append(timed(r, stream))
+        history_ms[(w, h)] = (float(np.median(off)), float(np.median(on)), float(np.min(on)))
+        del r, rh
 
     lines = [f"# Option aov and crtc_denoise on {name} (power limit {power})", "",
              f"`python scripts/bench_denoise.py` (frames {args.frames}, warm-up {args.warmup}, {args.runs} alternated windows).", "",
@@ -108,6 +127,11 @@ def main():
               "| size | median ms | min ms |", "|---|---|---|"]
     for (w, h), (med, mn) in denoise_ms.items():
         lines.append(f"| {w}x{h} | {med:.3f} | {mn:.3f} |")
+    lines += ["", "## crtc_denoise with denoise_history = 32 after a camera move, K = 5, alternated call by call with "
+              "history-off calls", "", "| size | history off, median ms | history on, median ms | history on, min ms | added |",
+              "|---|---|---|---|---|"]
+    for (w, h), (off, on, mn) in history_ms.items():
+        lines.append(f"| {w}x{h} | {off:.3f} | {on:.3f} | {mn:.3f} | {on - off:+.3f} ms |")
     text = "\n".join(lines) + "\n"
     print(text)
     if args.out:
