@@ -82,6 +82,28 @@ RenderCUDA::RenderCUDA(bool native_display_) : native_display(native_display_)
     if (denoise_history != 0 && !denoise) {
         throw std::runtime_error("crt_cuda: CRT_CUDA_DENOISE_HISTORY is the denoiser's history; it needs CRT_CUDA_DENOISE=1");
     }
+    // CRT_CUDA_ADAPTIVE=<threshold>: adaptive sampling (crtc_set_adaptive), with CRT_CUDA_ADAPTIVE_MIN_FRAMES (default 4)
+    // and CRT_CUDA_ADAPTIVE_MAX_FRAMES (default 0 = no cap)
+    const char *adaptive_env = std::getenv("CRT_CUDA_ADAPTIVE");
+    const bool adaptive = adaptive_env && *adaptive_env;
+    crtc_adaptive_params_t adaptive_params = {0.f, 4, 0};
+    if (adaptive) {
+        char *end = nullptr;
+        adaptive_params.threshold = std::strtof(adaptive_env, &end);
+        if (end == adaptive_env || *end != '\0') {
+            throw std::runtime_error(std::string("crt_cuda: cannot parse CRT_CUDA_ADAPTIVE='") + adaptive_env + "' as a threshold");
+        }
+        if (denoise) {
+            throw std::runtime_error("crt_cuda: CRT_CUDA_ADAPTIVE cannot be combined with CRT_CUDA_DENOISE=1 (the denoiser "
+                                     "assumes the same number of samples in every pixel)");
+        }
+        const long min_frames = env_or("CRT_CUDA_ADAPTIVE_MIN_FRAMES", 4), max_frames = env_or("CRT_CUDA_ADAPTIVE_MAX_FRAMES", 0);
+        if (min_frames < 0 || max_frames < 0) {
+            throw std::runtime_error("crt_cuda: CRT_CUDA_ADAPTIVE_MIN_FRAMES and CRT_CUDA_ADAPTIVE_MAX_FRAMES must not be negative");
+        }
+        adaptive_params.min_frames = static_cast<uint32_t>(min_frames);
+        adaptive_params.max_frames = static_cast<uint32_t>(max_frames);
+    }
     try {
         for (size_t i = 0; i < devices.size(); ++i) {
             crtc_renderer *r = nullptr;
@@ -99,6 +121,9 @@ RenderCUDA::RenderCUDA(bool native_display_) : native_display(native_display_)
             check(crtc_set_option(r, "aov", denoise ? 1 : 0));  // CRT_CUDA_DENOISE: first-hit AOVs for crtc_denoise
             if (denoise_history != 0) {
                 check(crtc_set_option(r, "denoise_history", denoise_history));  // (out of range: refused here)
+            }
+            if (adaptive) {
+                check(crtc_set_adaptive(r, &adaptive_params));  // (out of range: refused here)
             }
         }
     } catch (...) {

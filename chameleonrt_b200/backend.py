@@ -36,7 +36,7 @@ C_ABI_SYMBOLS = (
     "crtc_initialize", "crtc_set_scene", "crtc_render", "crtc_render_async", "crtc_sync", "crtc_read_accum", "crtc_get_stage_times",
     "crtc_get_counters", "crtc_get_scene_info", "crtc_trace_closest", "crtc_trace_any", "crtc_bench_trace",
     "crtc_local_buffers", "crtc_assemble_rank", "crtc_export_frame", "crtc_import_frame", "crtc_share_frame", "crtc_read_img", "crtc_frame_wait", "crtc_copy_img_to_array",
-    "crtc_read_aov", "crtc_denoise", "crtc_read_denoise_history",
+    "crtc_read_aov", "crtc_denoise", "crtc_read_denoise_history", "crtc_set_adaptive", "crtc_read_adaptive",
 )
 # Per-pixel layout of crtc_read_aov: name -> (first float, number of floats)
 AOV_LAYOUT = {"albedo": (0, 3), "coverage": (3, 1), "normal": (4, 3), "depth": (7, 1), "lum_m1": (8, 1), "lum_m2": (9, 1)}
@@ -50,6 +50,11 @@ class CDenoiseParams(C.Structure):
     """crtc_denoise_params_t"""
     _fields_ = [("iterations", C.c_int), ("sigma_luminance", C.c_float), ("sigma_normal", C.c_float),
                 ("sigma_depth", C.c_float)]
+
+
+class CAdaptiveParams(C.Structure):
+    """crtc_adaptive_params_t"""
+    _fields_ = [("threshold", C.c_float), ("min_frames", C.c_uint32), ("max_frames", C.c_uint32)]
 
 
 def lib_path() -> str:
@@ -98,6 +103,8 @@ def load_lib() -> C.CDLL:
     lib.crtc_read_aov.argtypes = [vp, vp]
     lib.crtc_denoise.argtypes = [vp, C.POINTER(CDenoiseParams), vp, vp, vp]
     lib.crtc_read_denoise_history.argtypes = [vp, vp]
+    lib.crtc_set_adaptive.argtypes = [vp, C.POINTER(CAdaptiveParams)]
+    lib.crtc_read_adaptive.argtypes = [vp, vp, vp]
     _lib = lib
     return lib
 
@@ -279,6 +286,24 @@ class RenderCUDA:
         a = np.zeros((self.height, self.width, HISTORY_FLOATS), dtype=np.float32)
         self._check(self.lib.crtc_read_denoise_history(self.h, a.ctypes.data))
         return {k: (a[:, :, o:o + n] if n > 1 else a[:, :, o]).copy() for k, (o, n) in HISTORY_LAYOUT.items()}
+
+    def set_adaptive(self, threshold: Optional[float], min_frames: int = 4, max_frames: int = 0) -> None:
+        """Adaptive sampling (crtc_set_adaptive): from the next render call on, 8x4 pixel blocks whose relative error is at
+        most ``threshold`` (after ``min_frames`` frames) stop tracing; ``max_frames`` > 0 caps every block's frames.
+        ``set_adaptive(None)`` turns it off."""
+        if threshold is None:
+            self._check(self.lib.crtc_set_adaptive(self.h, None))
+            return
+        prm = CAdaptiveParams(float(threshold), int(min_frames), int(max_frames))
+        self._check(self.lib.crtc_set_adaptive(self.h, C.byref(prm)))
+
+    def read_adaptive(self) -> dict:
+        """Per pixel (crtc_read_adaptive): ``samples`` (h, w) uint32, the samples accumulated, and ``error`` (h, w)
+        float32, the pixel error e_p the selection uses. Pixels of other ranks' tiles read 0."""
+        samples = np.zeros((self.height, self.width), dtype=np.uint32)
+        error = np.zeros((self.height, self.width), dtype=np.float32)
+        self._check(self.lib.crtc_read_adaptive(self.h, samples.ctypes.data, error.ctypes.data))
+        return {"samples": samples, "error": error}
 
     def stage_times(self) -> dict:
         a = np.zeros(len(STAGE_NAMES), dtype=np.float32)

@@ -42,12 +42,6 @@ inline void aov_launch(void (*kernel)(P...), unsigned grid, unsigned block, cuda
 #endif
 }
 
-// k_resolve's running mean: (x + n * acc) / (n + 1) for the frame with frame_id n
-CRT_D float aov_running_mean(float x, float acc, uint32_t n)
-{
-    return (x + (float)n * acc) / (float)(n + 1u);
-}
-
 // One thread per local pixel; the batch's frames * spp samples in sample order, with k_resolve's slot indexing.
 // Hit: base colour as k_shade unpacks it (same template branch), the TriShade normal face-forwarded as k_shade does
 // (render_embree.ispc:296-300), the hit distance. Miss: albedo = the miss shader's colour (a demodulated background

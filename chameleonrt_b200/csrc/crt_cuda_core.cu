@@ -16,6 +16,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/crt_cuda.h"
+#include "adaptive.cuh"
 #include "aov_denoise.cuh"
 #include "bvh8.h"
 #include "cuda_host_utils.h"
@@ -251,6 +252,49 @@ struct crtc_renderer {
         if (frame_id == 0) {
             throw std::runtime_error(std::string(what) + ": no frame has been rendered since the last reset");
         }
+    }
+
+    // Adaptive sampling (crtc_set_adaptive, adaptive.cuh). `adaptive` = the mode is set; `adaptive_epoch` = the per-block
+    // counts are in use, from the first adaptive wavefront after a reset until the next reset (switching the mode off in
+    // between keeps them, with every block active); `adaptive_base` = frame_id at that first wavefront, where the
+    // statistics start.
+    bool adaptive = false, adaptive_epoch = false;
+    crtc_adaptive_params_t adaptive_params{};
+    uint32_t adaptive_base = 0;
+    crt::AdaptiveState adaptive_state;
+    void set_adaptive(const crtc_adaptive_params_t *params)
+    {
+        if (!params) {
+            adaptive = false;
+            return;
+        }
+        if (aov_active) {
+            throw std::runtime_error("crtc_set_adaptive: adaptive sampling cannot be combined with option aov (the AOVs and the "
+                                     "denoiser assume the same number of samples in every pixel); this renderer was "
+                                     "initialized with aov = 1");
+        }
+        if (!std::isfinite(params->threshold) || params->threshold < 0.f) {
+            throw std::runtime_error("crtc_set_adaptive: threshold must be finite and >= 0");
+        }
+        if (params->min_frames < 1) {
+            throw std::runtime_error("crtc_set_adaptive: min_frames must be >= 1");
+        }
+        if (params->max_frames != 0 && params->max_frames < params->min_frames) {
+            throw std::runtime_error("crtc_set_adaptive: max_frames must be 0 (no cap) or >= min_frames");
+        }
+        adaptive = true;
+        adaptive_params = *params;
+    }
+    void read_adaptive(uint32_t *samples_out, float *error_out)
+    {
+        if (!adaptive_epoch || frame_id == 0) {
+            throw std::runtime_error("crtc_read_adaptive: no frame has been rendered with adaptive sampling since the last reset");
+        }
+        make_current();
+        if ((samples_out || error_out) && npx_local) {
+            adaptive_state.readout(frame_layout(), adaptive_base, samples_out, error_out, stream);
+        }
+        CUDA_CHECK(cudaGetLastError());
     }
 
     // frames: records of enqueued-but-not-collected frames, and a pool of reusable ones
@@ -615,6 +659,11 @@ struct crtc_renderer {
             throw std::runtime_error("initialize: option denoise_history needs option aov = 1 (the history is built from the "
                                      "first-hit AOVs)");
         }
+        if (aov && adaptive) {
+            throw std::runtime_error("initialize: option aov cannot be combined with adaptive sampling (the AOVs and the "
+                                     "denoiser assume the same number of samples in every pixel); turn it off with "
+                                     "crtc_set_adaptive(r, NULL) first");
+        }
         make_current();
         CUDA_CHECK(cudaStreamSynchronize(stream));
         unpin_img();             // (the caller's img buffer is reallocated with the new size)
@@ -645,6 +694,8 @@ struct crtc_renderer {
         } else {
             aov_state.release();
         }
+        adaptive_epoch = false;
+        adaptive_state.release();  // (sized by the first adaptive wavefront)
         share_seq = 0;
         CUDA_CHECK(cudaStreamSynchronize(stream));
     }
@@ -655,6 +706,7 @@ struct crtc_renderer {
     {
         make_current();
         frame_id = 0;
+        adaptive_epoch = false;
         auto_frames = 0;
         auto_decided = false;
         crt::SceneRecords rec;  // the device build fills rec.shading only
@@ -764,6 +816,7 @@ struct crtc_renderer {
         make_current();
         if (camera_changed) {
             frame_id = 0;  // render_embree.cpp:145-147
+            adaptive_epoch = false;
         }
         const crt::ViewParams view = crt::make_view_params(pos, dir, up, fovy, fb_w, fb_h, frame_id);
         if (frame_id == 0) {  // the first frame since a reset starts a new epoch (crtc_denoise's history)
@@ -803,6 +856,27 @@ struct crtc_renderer {
         if (count_traversal) {
             CUDA_CHECK(cudaMemsetAsync(d_trav_counters.ptr, 0, 4 * sizeof(unsigned long long), stream));
         }
+        // adaptive sampling: which blocks render how many of this wavefront's frames, decided once per call
+        const bool adaptive_frame = adaptive || adaptive_epoch;
+        crt::AdaptiveSelect sel{};
+        if (adaptive_frame) {
+            sel.reset = adaptive_epoch ? 0u : 1u;
+            if (!adaptive_epoch) {
+                adaptive_epoch = true;
+                adaptive_base = frame_id;
+                adaptive_state.ensure(npx_local);
+            }
+            sel.frames = num_frames;
+            sel.stat_base = adaptive_base;
+            // The any_far_first trial compares the traversal times of two blocking frames, which must see the same work.
+            sel.all_active = (!adaptive || (any_far_first == 2 && !auto_decided && blocking)) ? 1u : 0u;
+            if (adaptive) {
+                sel.threshold = adaptive_params.threshold;
+                sel.min_frames = adaptive_params.min_frames;
+                sel.max_frames = adaptive_params.max_frames;
+            }
+        }
+        const crt::AdaptiveFrame ad = adaptive_state.frame(adaptive_base);
         if (npaths) {
             const unsigned g256 = (unsigned)((npaths + 255) / 256);
             // k_nee_resolve strides over its queue: two waves of resident blocks cover any queue length
@@ -811,7 +885,13 @@ struct crtc_renderer {
             }
             const unsigned g128 = (unsigned)((npaths + 127) / 128);
             const unsigned g_nee = (unsigned)std::min<size_t>((npaths + 255) / 256, (size_t)num_sms * 8 * 2);
-            crt::k_raygen<<<g256, 256, 0, stream>>>(view, fl, ps);
+            if (adaptive_frame) {  // (its time counts as raygen)
+                adaptive_state.select(fl, sel, stream);
+                rec.launches += 1;
+                adaptive_state.raygen(g256, view, fl, ps, ad, stream);
+            } else {
+                crt::k_raygen<<<g256, 256, 0, stream>>>(view, fl, ps);
+            }
             rec.mark(stream, kStRaygen);
             // closest hit of the primary rays, then per bounce: shade -> one traversal launch for this
             // bounce's shadow rays AND the next bounce's continuation rays -> NEE resolve
@@ -864,8 +944,13 @@ struct crtc_renderer {
                 }
                 arrive = peer_sync_words() + rank;
             }
-            crt::k_resolve<<<gpx, 256, 0, stream>>>(fl, ps, frame_id, d_accum_local.ptr, d_img_local.ptr, full_accum, full_img,
-                                                   d_done_counter.ptr, arrive, share_seq + 1u);
+            if (adaptive_frame) {  // (only active pixels are stored into a shared frame: it holds the others already)
+                adaptive_state.resolve(gpx, fl, ps, frame_id, d_accum_local.ptr, d_img_local.ptr, full_accum, full_img,
+                                       d_done_counter.ptr, arrive, share_seq + 1u, ad, stream);
+            } else {
+                crt::k_resolve<<<gpx, 256, 0, stream>>>(fl, ps, frame_id, d_accum_local.ptr, d_img_local.ptr, full_accum, full_img,
+                                                       d_done_counter.ptr, arrive, share_seq + 1u);
+            }
             rec.launches += 1;
             if (aov_active) {  // (counted in the resolve stage)
                 aov_state.launch_moments(fl, ps, frame_id, stream);
@@ -1530,6 +1615,16 @@ int crtc_read_denoise_history(crtc_renderer *r, float *out)
         }
         r->read_denoise_history(out);
     })
+}
+
+int crtc_set_adaptive(crtc_renderer *r, const crtc_adaptive_params_t *params)
+{
+    CRTC_TRY({ require_renderer(r); r->set_adaptive(params); })
+}
+
+int crtc_read_adaptive(crtc_renderer *r, uint32_t *samples_out, float *error_out)
+{
+    CRTC_TRY({ require_renderer(r); r->read_adaptive(samples_out, error_out); })
 }
 
 int crtc_get_stage_times(crtc_renderer *r, float *ms_out, int n)

@@ -160,8 +160,20 @@ __device__ __forceinline__ uint32_t warp_append(uint32_t *counter, bool pred)
     return base + (uint32_t)__popc(mask & ((1u << lane) - 1u));
 }
 
+// Adaptive sampling (crtc_set_adaptive, adaptive.cuh): the per-block selection k_adaptive_select made for this wavefront.
+// Block b = local pixels 32b .. 32b+31 (one 8x4 screen block, one warp of k_raygen and k_resolve): sel[b] = {c_b, n_b}, the
+// frames the block had accumulated before this wavefront and the frames it renders in it. moments[lp] = (m1, m2), the
+// running means of L and L^2, whose count starts at stat_base.
+struct AdaptiveFrame {
+    const uint2 *sel;
+    float2 *moments;
+    uint32_t stat_base;
+};
+
 // ---------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_raygen(ViewParams view, FrameLayout f, PathState ps)
+// ADAPTIVE: only the first n_b frames of each block are enqueued, seeded as frames c_b, c_b + 1, ... of the uniform render.
+template <bool ADAPTIVE = false>
+__global__ void __launch_bounds__(256) k_raygen(ViewParams view, FrameLayout f, PathState ps, AdaptiveFrame ad = AdaptiveFrame{})
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     const uint32_t npaths = f.npx_local * f.spp * f.frames;
@@ -169,11 +181,18 @@ __global__ void __launch_bounds__(256) k_raygen(ViewParams view, FrameLayout f, 
     if (i < npaths) {
         // sample index over the batch: frame (view.frame_id + s / spp), sample s % spp of it
         const uint32_t lp = i % f.npx_local, s = i / f.npx_local;
+        uint32_t first = view.frame_id;
+        bool active = true;
+        if (ADAPTIVE) {  // (warp-uniform: npx_local is a multiple of 32, so a warp's 32 paths are one block's)
+            const uint2 sel = ad.sel[lp >> 5];
+            first = sel.x;
+            active = s < sel.y * f.spp;
+        }
         uint32_t x, y;
-        if (local_pixel_coords(f, lp, x, y)) {
+        if (active && local_pixel_coords(f, lp, x, y)) {
             valid = true;
             // render_embree.ispc:213-232; (frame_id + k) * spp + 1 + (s - k * spp) == frame_id * spp + 1 + s
-            uint32_t rng = get_rng(x + y * (uint32_t)f.fb_w, view.frame_id * f.spp + 1u + s);
+            uint32_t rng = get_rng(x + y * (uint32_t)f.fb_w, first * f.spp + 1u + s);
             const float px_x = ((float)x + lcg_randomf(rng)) / (float)(uint32_t)f.fb_w;
             const float px_y = ((float)y + lcg_randomf(rng)) / (float)(uint32_t)f.fb_h;
             const float3 dir = normalize(mk3(view.dir_du.x * px_x + view.dir_dv.x * px_y + view.dir_top_left.x,
@@ -918,26 +937,56 @@ __global__ void __launch_bounds__(32) k_set_word(uint32_t *word, uint32_t v)
     }
 }
 
+// k_resolve's running mean: (x + n * acc) / (n + 1) for the frame with frame_id n
+CRT_D float aov_running_mean(float x, float acc, uint32_t n)
+{
+    return (x + (float)n * acc) / (float)(n + 1u);
+}
+
 // render_embree.ispc:339-353 (sample mean + running mean) and :358-370 (sRGB8)
+// ADAPTIVE: each block folds its n_b frames with its own count c_b in place of frame_id, and the luminance moments with
+// them (k_aov_moments' fold); a block with n_b = 0 leaves every buffer of its pixels untouched.
+template <bool ADAPTIVE = false>
 __global__ void __launch_bounds__(256) k_resolve(FrameLayout f, PathState ps, uint32_t frame_id, float *accum_local,
                                                 uint32_t *img_local, float *accum_full, uint32_t *img_full,
-                                                uint32_t *done_counter, uint32_t *arrive_word, uint32_t seq)
+                                                uint32_t *done_counter, uint32_t *arrive_word, uint32_t seq,
+                                                AdaptiveFrame ad = AdaptiveFrame{})
 {
     const uint32_t lp = blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t x, y;
-    if (lp < f.npx_local && local_pixel_coords(f, lp, x, y)) {
+    uint32_t first = frame_id, frames = f.frames;
+    if (ADAPTIVE && lp < f.npx_local) {
+        const uint2 sel = ad.sel[lp >> 5];
+        first = sel.x;
+        frames = sel.y;
+    }
+    if (lp < f.npx_local && (!ADAPTIVE || frames != 0u) && local_pixel_coords(f, lp, x, y)) {
         // the frames of the batch are folded into the running mean one after the other, exactly as if
         // they had been rendered by separate calls
         float3 illum = mk3(accum_local[3 * (size_t)lp], accum_local[3 * (size_t)lp + 1], accum_local[3 * (size_t)lp + 2]);
-        for (uint32_t k = 0; k < f.frames; ++k) {
+        float2 m = ADAPTIVE ? ad.moments[lp] : make_float2(0.f, 0.f);
+        for (uint32_t k = 0; k < frames; ++k) {
             const float3 accum = illum;
             illum = mk3(0.f);
+            float s1 = 0.f, s2 = 0.f;
             for (uint32_t s = 0; s < f.spp; ++s) {
                 const float4 r = ps.radiance[(size_t)(k * f.spp + s) * f.npx_local + lp];
                 illum = illum + mk3(r.x, r.y, r.z);
+                if (ADAPTIVE) {
+                    const float l = luminance(mk3(r.x, r.y, r.z));
+                    s1 += l;
+                    s2 += l * l;
+                }
             }
             illum = illum / (float)f.spp;
-            illum = (illum + (float)(frame_id + k) * accum) / (float)(frame_id + k + 1u);
+            illum = (illum + (float)(first + k) * accum) / (float)(first + k + 1u);
+            if (ADAPTIVE) {
+                m.x = aov_running_mean(s1 / (float)f.spp, m.x, first + k - ad.stat_base);
+                m.y = aov_running_mean(s2 / (float)f.spp, m.y, first + k - ad.stat_base);
+            }
+        }
+        if (ADAPTIVE) {
+            ad.moments[lp] = m;
         }
         accum_local[3 * (size_t)lp] = illum.x;
         accum_local[3 * (size_t)lp + 1] = illum.y;

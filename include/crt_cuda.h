@@ -152,7 +152,9 @@ int crtc_render(crtc_renderer *r, const float *pos, const float *dir, const floa
  * result) — which keeps a GPU that owns only part of the image busy. crtc_sync waits for all such frames and returns
  * their totals: `total` (render_time = sum of per-frame device times, num_rays = sum),
  * `stage_ms_sum` (7 floats, as crtc_get_stage_times), `counters_sum` (8, as crtc_get_counters),
- * `num_frames`; any of them may be NULL. The accumulation semantics are those of crtc_render. */
+ * `num_frames`; any of them may be NULL. The accumulation semantics are those of crtc_render. With adaptive sampling
+ * (crtc_set_adaptive) a call selects its active blocks once: every pixel still holds the uniform render's result at its
+ * own count, but which blocks advance may differ from num_frames separate calls. */
 int crtc_render_async(crtc_renderer *r, const float *pos, const float *dir, const float *up, float fovy,
                       int camera_changed, uint32_t num_frames);
 int crtc_sync(crtc_renderer *r, crt_render_stats_t *total, float *stage_ms_sum, uint64_t *counters_sum,
@@ -296,6 +298,48 @@ int crtc_denoise(crtc_renderer *r, const crtc_denoise_params_t *params, float *r
 /* Option "denoise_history": `cur`, fb_width*fb_height*10 floats, row-major (I.rgb, M1, M2, n, z, nhat.xyz per pixel, as
  * in crtc_denoise). Fails if the option is off or no crtc_denoise has run since the last reset. */
 int crtc_read_denoise_history(crtc_renderer *r, float *out);
+
+typedef struct crtc_adaptive_params_t {
+    float threshold;     /* a block stops when its error E_b is <= threshold (finite, >= 0) */
+    uint32_t min_frames; /* >= 1: frames every block renders before its error is trusted */
+    uint32_t max_frames; /* 0 = no cap, else >= min_frames: no block renders more frames */
+} crtc_adaptive_params_t;
+
+/* Adaptive sampling: pixel blocks whose noise estimate has converged stop tracing. Off by default; params = NULL turns it
+ * off. Takes effect at the next crtc_render / crtc_render_async call. Out-of-range params are an error, and so is a
+ * renderer initialized with option "aov" (the AOVs and the denoiser assume the same samples in every pixel);
+ * crtc_initialize with option aov fails while the mode is set.
+ *   Block. Block b is the 32 local pixels 32b .. 32b+31 in local order: an 8x4 screen rectangle aligned to the 64x64 tile
+ *   grid. It keeps c_b, the frames it has accumulated since the last reset (crtc_initialize, crtc_set_scene, a render
+ *   with camera_changed), and per pixel m1, m2: the running means of L and L^2 over the samples (L and the fold of
+ *   crtc_read_aov's lum_m1 / lum_m2, with the block's count in place of the frame index), so that they equal lum_m1 /
+ *   lum_m2 of a uniform render with option aov at the same count.
+ *   Pixel error. With N = c_b * spp: e_p = sqrt(max(0, m2 - m1^2) / (N * max(m1, 1e-4))), in float (+inf where N = 0): the
+ *   standard error of the mean relative to sqrt(luminance). Block error E_b = the max of e_p over its in-frame pixels.
+ *   Selection, once per crtc_render / crtc_render_async call (one wavefront of F frames), from the state at that moment:
+ *   a block with no in-frame pixel gets n_b = 0; otherwise n_b = F if c_b < min_frames, or E_b > threshold, or the call is
+ *   a crtc_render while option any_far_first = 2 has not decided (its trial compares the traversal time of two frames,
+ *   which must see the same work); else n_b = 0. With max_frames > 0, n_b is capped at max_frames - c_b.
+ *   Rendering. Only the samples of a block's frames k < n_b are traced, seeded as frame c_b + k of the uniform render;
+ *   the block folds them into accum with c_b in place of the frame index, then c_b += n_b. A block with n_b = 0 leaves
+ *   its accum, img and moments, and its pixels of a shared full frame, untouched.
+ *   Guarantee. A pixel whose block has count c holds the accum and img that a uniform render with the same camera holds
+ *   after c frames, bit for bit.
+ *   Epochs. The counts are used from the first adaptive call after a reset until the next reset. Switching the mode off
+ *   in between keeps them and makes every in-frame block active (n_b = F), so the guarantee still holds. Switching it on
+ *   after c0 uniform frames of an epoch starts every count at c0 and the moments with that call: there N = (c_b - c0) *
+ *   spp, the moments fold with c_b - c0, and min_frames counts from c0.
+ *   Batches. A crtc_render_async call of F frames is one selection: per pixel the result is that of c_b frames, as above,
+ *   but which blocks advance may differ from F separate calls.
+ *   Stats. num_rays and counter [5] (paths started) count what was traced; counter [2] (launches) grows by 1 per call
+ *   for the selection kernel. Memory: 12 B per block and 8 B per local pixel, + 8 B per framebuffer pixel for the
+ *   first crtc_read_adaptive. */
+int crtc_set_adaptive(crtc_renderer *r, const crtc_adaptive_params_t *params);
+
+/* Adaptive sampling: per pixel, row-major fb_width*fb_height, the samples accumulated (c_b * spp) and e_p; either output
+ * may be NULL. Pixels of tiles this renderer does not own are left untouched, as crtc_read_img leaves them. Fails if no
+ * frame has been rendered with adaptive sampling since the last reset. */
+int crtc_read_adaptive(crtc_renderer *r, uint32_t *samples_out, float *error_out);
 
 #ifdef __cplusplus
 }
