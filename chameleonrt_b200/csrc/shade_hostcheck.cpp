@@ -40,127 +40,36 @@ using std::min;
 
 #include "shade_math.cuh"
 
-namespace {
-crt::DisneyMaterial material_from16(const float *m)
-{
-    crt::DisneyMaterial d;
-    d.base_color = crt::mk3(m[0], m[1], m[2]);
-    d.metallic = m[3];
-    d.specular = m[4];
-    d.roughness = m[5];
-    d.specular_tint = m[6];
-    d.anisotropy = m[7];
-    d.sheen = m[8];
-    d.sheen_tint = m[9];
-    d.clearcoat = m[10];
-    d.clearcoat_gloss = m[11];
-    d.ior = m[12];
-    d.specular_transmission = m[13];
-    return d;
-}
-crt::QuadLight light_from20(const float *l)
-{
-    crt::QuadLight q;
-    q.emission = crt::mk3(l[0], l[1], l[2]);
-    q.position = crt::mk3(l[4], l[5], l[6]);
-    q.normal = crt::mk3(l[8], l[9], l[10]);
-    q.v_x = crt::mk3(l[12], l[13], l[14]);
-    q.width = l[15];
-    q.v_y = crt::mk3(l[16], l[17], l[18]);
-    q.height = l[19];
-    return q;
-}
-}  // namespace
+#include "shade_kat.h"
 
 extern "C" {
 
 void shadekat_rng(uint32_t pixel_id, uint32_t frame_id, uint32_t n, uint32_t *states, float *floats)
 {
-    uint32_t rng = crt::get_rng(pixel_id, frame_id);
-    for (uint32_t i = 0; i < n; ++i) {
-        floats[i] = crt::lcg_randomf(rng);
-        states[i] = rng;
-    }
+    crt::kat_rng(pixel_id, frame_id, n, states, floats);
 }
 // out: f.xyz, pdf
 void shadekat_disney_eval(const float *mat16, const float *n, const float *w_o, const float *w_i, float *out4)
 {
-    using namespace crt;
-    const DisneyMaterial mat = material_from16(mat16);
-    const float3 nn = mk3(n[0], n[1], n[2]);
-    float3 v_x, v_y;
-    ortho_basis(v_x, v_y, nn);
-    const float3 wo = mk3(w_o[0], w_o[1], w_o[2]), wi = mk3(w_i[0], w_i[1], w_i[2]);
-    const float3 f = disney_brdf(mat, nn, wo, wi, v_x, v_y);
-    out4[0] = f.x;
-    out4[1] = f.y;
-    out4[2] = f.z;
-    out4[3] = disney_pdf(mat, nn, wo, wi, v_x, v_y);
+    crt::kat_disney_eval(mat16, n, w_o, w_i, out4);
 }
 // rng_state in/out; out: f.xyz, pdf, w_i.xyz
 void shadekat_disney_sample(const float *mat16, const float *n, const float *w_o, uint32_t *rng_state, float *out7)
 {
-    using namespace crt;
-    const DisneyMaterial mat = material_from16(mat16);
-    const float3 nn = mk3(n[0], n[1], n[2]);
-    float3 v_x, v_y;
-    ortho_basis(v_x, v_y, nn);
-    uint32_t rng = *rng_state;
-    float3 w_i = mk3(0.f);
-    float pdf = 0.f;
-    const float3 f = sample_disney_brdf(mat, nn, mk3(w_o[0], w_o[1], w_o[2]), v_x, v_y, rng, w_i, pdf);
-    *rng_state = rng;
-    out7[0] = f.x;
-    out7[1] = f.y;
-    out7[2] = f.z;
-    out7[3] = pdf;
-    out7[4] = w_i.x;
-    out7[5] = w_i.y;
-    out7[6] = w_i.z;
+    crt::kat_disney_sample(mat16, n, w_o, rng_state, out7);
 }
 // light20: QuadLight; out: sample_pos.xyz, pdf(p = sample_pos, dir), hit flag, t, hit_pos.xyz
 void shadekat_light(const float *light20, const float *s2, const float *orig, const float *dir, float *out9)
 {
-    using namespace crt;
-    const QuadLight l = light_from20(light20);
-    const float3 p = sample_quad_light_position(l, s2[0], s2[1]);
-    const float3 o = mk3(orig[0], orig[1], orig[2]), d = mk3(dir[0], dir[1], dir[2]);
-    out9[0] = p.x;
-    out9[1] = p.y;
-    out9[2] = p.z;
-    out9[3] = quad_light_pdf(l, p, d);
-    float t = 0.f;
-    float3 lp = mk3(0.f);
-    const bool hit = quad_intersect(l, o, d, t, lp);
-    out9[4] = hit ? 1.f : 0.f;
-    out9[5] = hit ? t : 0.f;
-    out9[6] = hit ? lp.x : 0.f;
-    out9[7] = hit ? lp.y : 0.f;
-    out9[8] = hit ? lp.z : 0.f;
+    crt::kat_light(light20, s2, orig, dir, out9);
 }
 // data: w*h*channels bytes, expanded to the device's RGBA8 arena layout (host_scene.cpp) before sampling
 void shadekat_texture(const uint8_t *data, int w, int h, int channels, const float *uv, int n, float *out4n)
 {
-    using namespace crt;
-    std::vector<uint32_t> texels((size_t)w * h);
-    for (size_t px = 0; px < (size_t)w * h; ++px) {
-        uint32_t c[4] = {0, 0, 0, 0};
-        for (int k = 0; k < channels; ++k) {
-            c[k] = data[px * channels + k];
-        }
-        texels[px] = c[0] | (c[1] << 8) | (c[2] << 16) | (c[3] << 24);
-    }
-    DevTex t;
-    t.offset = 0;
-    t.width = w;
-    t.height = h;
-    t.pad = 0;
+    const std::vector<uint32_t> texels = crt::rgba8_arena(data, w, h, channels);
+    const crt::DevTex t{0u, w, h, 0};
     for (int i = 0; i < n; ++i) {
-        const float4 c = texture_rgba(texels.data(), t, make_float2(uv[2 * i], uv[2 * i + 1]));
-        out4n[4 * i] = c.x;
-        out4n[4 * i + 1] = c.y;
-        out4n[4 * i + 2] = c.z;
-        out4n[4 * i + 3] = c.w;
+        crt::kat_texture(texels.data(), t, uv[2 * i], uv[2 * i + 1], out4n + 4 * i);
     }
 }
 // the byte -> [0, 1] table texel channels are converted with (kByteToUnit, read through byte_to_unit)
@@ -175,42 +84,111 @@ void shadekat_byte_to_unit(float *out256)
 void shadekat_unpack_material(const float *materials, uint32_t id, const uint32_t *texels, const int32_t *tex,
                               const float *uv, int n, float *out14n)
 {
-    using namespace crt;
-    const TexSource ts{texels, reinterpret_cast<const DevTex *>(tex), nullptr};
+    const crt::TexSource ts{texels, reinterpret_cast<const crt::DevTex *>(tex), nullptr};
     for (int i = 0; i < n; ++i) {
-        DisneyMaterial m;
-        unpack_material<false>(m, reinterpret_cast<const float4 *>(materials), id, make_float2(uv[2 * i], uv[2 * i + 1]),
-                               ts);
-        const float v[14] = {m.base_color.x, m.base_color.y, m.base_color.z, m.metallic, m.specular, m.roughness,
-                             m.specular_tint, m.anisotropy, m.sheen, m.sheen_tint, m.clearcoat, m.clearcoat_gloss, m.ior,
-                             m.specular_transmission};
-        std::memcpy(out14n + 14 * i, v, sizeof v);
+        crt::kat_unpack_material(materials, id, ts, uv[2 * i], uv[2 * i + 1], out14n + 14 * i);
     }
 }
 void shadekat_miss(const float *dirs, int n, float *out3n)
 {
     for (int i = 0; i < n; ++i) {
-        const float3 c = crt::miss_shader(crt::mk3(dirs[3 * i], dirs[3 * i + 1], dirs[3 * i + 2]));
-        out3n[3 * i] = c.x;
-        out3n[3 * i + 1] = c.y;
-        out3n[3 * i + 2] = c.z;
+        crt::kat_miss(dirs + 3 * i, out3n + 3 * i);
     }
 }
 void shadekat_ortho_basis(const float *n, float *out6)
 {
-    float3 vx, vy;
-    crt::ortho_basis(vx, vy, crt::mk3(n[0], n[1], n[2]));
-    out6[0] = vx.x;
-    out6[1] = vx.y;
-    out6[2] = vx.z;
-    out6[3] = vy.x;
-    out6[4] = vy.y;
-    out6[5] = vy.z;
+    crt::kat_ortho_basis(n, out6);
 }
 void shadekat_srgb8(const float *x, int n, uint8_t *out)
 {
     for (int i = 0; i < n; ++i) {
         out[i] = (uint8_t)crt::float_to_srgb8(x[i]);
     }
+}
+
+// ---- batched: n inputs, n outputs. libcrt_shade_devcheck.so exports the same names and signatures (the same
+// per-input functions, one CUDA thread each), so that one test runs against either build (tests/test_shade_device.py).
+// Each returns 0 (the device build: a CUDA error code). ----
+int shadekat_rng_n(const uint32_t *pixel_ids, const uint32_t *frame_ids, int n, int k, uint32_t *states, float *floats)
+{
+    for (int i = 0; i < n; ++i) {
+        crt::kat_rng(pixel_ids[i], frame_ids[i], (uint32_t)k, states + (size_t)k * i, floats + (size_t)k * i);
+    }
+    return 0;
+}
+// one lcg_randomf per state, in place
+int shadekat_lcg_n(uint32_t *states, int n, float *floats)
+{
+    for (int i = 0; i < n; ++i) {
+        floats[i] = crt::lcg_randomf(states[i]);
+    }
+    return 0;
+}
+int shadekat_disney_eval_n(const float *mat16n, const float *n3n, const float *w_o3n, const float *w_i3n, int n, float *out4n)
+{
+    for (int i = 0; i < n; ++i) {
+        crt::kat_disney_eval(mat16n + 16 * i, n3n + 3 * i, w_o3n + 3 * i, w_i3n + 3 * i, out4n + 4 * i);
+    }
+    return 0;
+}
+int shadekat_disney_sample_n(const float *mat16n, const float *n3n, const float *w_o3n, uint32_t *rng_n, int n,
+                             float *out7n)
+{
+    for (int i = 0; i < n; ++i) {
+        crt::kat_disney_sample(mat16n + 16 * i, n3n + 3 * i, w_o3n + 3 * i, rng_n + i, out7n + 7 * i);
+    }
+    return 0;
+}
+int shadekat_light_n(const float *light20, const float *s2n, const float *orig3n, const float *dir3n, int n, float *out9n)
+{
+    for (int i = 0; i < n; ++i) {
+        crt::kat_light(light20, s2n + 2 * i, orig3n + 3 * i, dir3n + 3 * i, out9n + 9 * i);
+    }
+    return 0;
+}
+int shadekat_texture_n(const uint8_t *data, int w, int h, int channels, const float *uv, int n, float *out4n)
+{
+    shadekat_texture(data, w, h, channels, uv, n, out4n);
+    return 0;
+}
+// n_materials, n_texels, n_tex: the lengths of the three tables (the device build copies them)
+int shadekat_unpack_material_n(const float *materials, int n_materials, uint32_t id, const uint32_t *texels, int n_texels,
+                               const int32_t *tex, int n_tex, const float *uv, int n, float *out14n)
+{
+    (void)n_materials, (void)n_texels, (void)n_tex;
+    shadekat_unpack_material(materials, id, texels, tex, uv, n, out14n);
+    return 0;
+}
+int shadekat_miss_n(const float *dirs, int n, float *out3n)
+{
+    shadekat_miss(dirs, n, out3n);
+    return 0;
+}
+int shadekat_ortho_basis_n(const float *n3n, int n, float *out6n)
+{
+    for (int i = 0; i < n; ++i) {
+        crt::kat_ortho_basis(n3n + 3 * i, out6n + 6 * i);
+    }
+    return 0;
+}
+int shadekat_srgb8_n(const float *x, int n, uint8_t *out)
+{
+    shadekat_srgb8(x, n, out);
+    return 0;
+}
+int shadekat_schlick_n(const float *cos_theta, int n, float *out)
+{
+    for (int i = 0; i < n; ++i) {
+        out[i] = crt::schlick_weight(cos_theta[i]);
+    }
+    return 0;
+}
+// fn: crt::KatMath (sinf, cosf, powf, logf, atan2f, acosf); y is read by powf and atan2f only
+int shadekat_math_n(int fn, const float *x, const float *y, int n, float *out)
+{
+    for (int i = 0; i < n; ++i) {
+        out[i] = crt::kat_math(fn, x[i], y ? y[i] : 0.f);
+    }
+    return 0;
 }
 }

@@ -143,6 +143,15 @@ constexpr ByteToUnit make_byte_to_unit()
 __device__ const ByteToUnit kByteToUnit = make_byte_to_unit();
 CRT_D float byte_to_unit(uint32_t q) { return __ldg(kByteToUnit.v + q); }
 
+// (int)x as x86-64 converts it (cvttss2si): truncation toward zero, and INT_MIN for NaN and for every x outside
+// [-2^31, 2^31). The reference, the oracle and the host builds of this file convert texel coordinates that way; the
+// device's own conversion saturates and maps NaN to 0, which for a finite uv*width >= 2^31 picks texel column
+// INT_MAX mod width instead of INT_MIN mod width.
+CRT_D int float_to_int_x86(float x)
+{
+    return (x >= -2147483648.f && x < 2147483648.f) ? (int)x : INT32_MIN;
+}
+
 // The four texel words under the bilinear footprint of uv and the weights of the filter (texture2d.ih:13-83).
 struct TexelQuad {
     uint32_t p00, p10, p01, p11;
@@ -155,8 +164,8 @@ CRT_D TexelQuad texel_quad(const uint32_t *__restrict__ texels, const DevTex t, 
     TexelQuad q;
     q.tx = ux - floorf(ux);
     q.ty = uy - floorf(uy);
-    const int x0 = modi((int)ux, t.width), y0 = modi((int)uy, t.height);
-    const int x1 = modi((int)(ux + 1.f), t.width), y1 = modi((int)(uy + 1.f), t.height);
+    const int x0 = modi(float_to_int_x86(ux), t.width), y0 = modi(float_to_int_x86(uy), t.height);
+    const int x1 = modi(float_to_int_x86(ux + 1.f), t.width), y1 = modi(float_to_int_x86(uy + 1.f), t.height);
     const uint32_t *const base = texels + t.offset;
     q.p00 = __ldg(base + (uint32_t)(y0 * t.width + x0));
     q.p10 = __ldg(base + (uint32_t)(y0 * t.width + x1));
@@ -289,8 +298,9 @@ CRT_D float power_heuristic(float n_f, float pdf_f, float n_g, float pdf_g)
 }
 // disney_bsdf.ih:74-76 is pow(saturate(1 - cos_theta), 5). Evaluated here as m^2 * m^2 * m: powf is
 // ~100 instructions and this weight is needed ~10 times per shaded hit (it was about a third of
-// k_shade's instructions); the product is within 2 ulp of powf (the reference's own ISPC pow under
-// --opt=fast-math is no closer). One of the two documented arithmetic deviations (DESIGN.md §4).
+// k_shade's instructions); the product is within 3 ulp of the exact m^5 (2.92 ulp at most over every float
+// cos_theta in [0, 1]: tests/test_shade_device.py), pow within half an ulp; the reference's own ISPC pow under
+// --opt=fast-math is no closer. One of the two documented arithmetic deviations (DESIGN.md §4).
 CRT_D float schlick_weight(float cos_theta)
 {
     const float m = saturate(1.f - cos_theta);

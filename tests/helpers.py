@@ -177,3 +177,25 @@ def synthetic_material_scene(spp=1):
                   lights=[default_obj_light()], samples_per_pixel=spp)
     cam = dict(eye=(0.3, 1.6, 4.2), center=(0.0, 0.6, 0.0), up=(0.0, 1.0, 0.0), fov_y=50.0)
     return scene, cam
+
+
+def huge_uv_scene(spp=1):
+    """A textured quad whose uvs put uv.x * width between 2^31 and 2^32 texels: the texel index conversion is out of int
+    range, and texture2d.ih's x86 conversion (INT_MIN) reads column 0 of the 4-wide texture; each column has its own
+    colour, so a different conversion shows in the albedo."""
+    from chameleonrt_b200.scene import (SRGB, DisneyMaterial, Geometry, Image, Instance, Mesh, ParameterizedMesh, Scene,
+                                        default_obj_light, textured_param)
+
+    img = np.zeros((4, 4, 3), np.uint8)
+    img[:, :, 0] = np.array([200, 30, 90, 250], np.uint8)[None, :]  # red: per column
+    img[:, :, 1] = np.array([40, 120, 180, 240], np.uint8)[:, None]  # green: per row
+    img[:, :, 2] = 60
+    verts = np.array([[-1, -1, 0], [1, -1, 0], [1, 1, 0], [-1, 1, 0]], np.float32)
+    uvs = np.array([[2.0**29, 0.0], [2.0**30 - 64, 0.0], [2.0**30 - 64, 1.0], [2.0**29, 1.0]], np.float32)
+    geom = Geometry(vertices=verts, indices=np.array([[0, 1, 2], [0, 2, 3]], np.uint32), uvs=uvs)
+    scene = Scene(meshes=[Mesh([geom])], parameterized_meshes=[ParameterizedMesh(0, [0])],
+                  instances=[Instance(np.eye(4, dtype=np.float32), 0)],
+                  materials=[DisneyMaterial(base_color=(textured_param(0), 0.5, 0.5), roughness=0.5)],
+                  textures=[Image("columns", img, SRGB)], lights=[default_obj_light()], samples_per_pixel=spp)
+    cam = dict(eye=(0.0, 0.0, 3.0), center=(0.0, 0.0, 0.0), up=(0.0, 1.0, 0.0), fov_y=50.0)
+    return scene, cam

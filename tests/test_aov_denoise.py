@@ -18,7 +18,7 @@ import sys
 import numpy as np
 import pytest
 
-from helpers import camera_for, synthetic_material_scene
+from helpers import camera_for, huge_uv_scene, synthetic_material_scene
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "chameleonrt_b200", "csrc")
@@ -450,7 +450,8 @@ def check_errors(mods):
 def test_aov_content_on_the_emulated_renderer(emu, shade, spp):
     from chameleonrt_b200.scenes import cornell_box
 
-    for scene, cam, (w, h) in ((*cornell_box(spp=spp), (40, 24)), (*synthetic_material_scene(spp=spp), (40, 24))):
+    for scene, cam, (w, h) in ((*cornell_box(spp=spp), (40, 24)), (*synthetic_material_scene(spp=spp), (40, 24)),
+                               (*huge_uv_scene(spp=spp), (24, 16))):
         check_aov_content(emu, shade, scene, cam, w, h, frames=2)
 
 
@@ -521,6 +522,8 @@ def test_aov_content_cornell(gpu, shade):
 
     for spp in (1, 2):
         check_aov_content(gpu, shade, *cornell_box(spp=spp), 128, 96, frames=2)
+        # uv * width past 2^31 texels: the texel index the host conversion gives (shade_math.cuh: float_to_int_x86)
+        check_aov_content(gpu, shade, *huge_uv_scene(spp=spp), 64, 48, frames=2)
 
 
 @pytest.mark.gpu
