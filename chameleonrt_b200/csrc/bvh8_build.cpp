@@ -749,7 +749,7 @@ void assign_slots(const std::vector<B2Node> &n2, NodePlan &pl)
                 if (pl.slot_child[s] >= 0) {
                     continue;
                 }
-                if (cst[c][s] < best) {
+                if (cst[c][s] < best || bc < 0) {  // (the first candidate is taken whatever its cost, as on the device)
                     best = cst[c][s];
                     bc = c;
                     bs = s;

@@ -130,6 +130,13 @@ __global__ void __launch_bounds__(kBuildBlock) k_flatten(const DevSegment *segs,
         r[1] = w2o[4] * n[0] + w2o[5] * n[1] + w2o[6] * n[2];
         r[2] = w2o[8] * n[0] + w2o[9] * n[1] + w2o[10] * n[2];
         dev_normalize3(r);
+        for (int k = 0; k < 3; ++k) {
+            // a zero-area triangle's normal is 0 * inf: store the NaN flatten_scene gets on x86 (0xffc00000), not the
+            // GPU's canonical 0x7fffffff, so that the records are the same bits on both paths
+            if (r[k] != r[k]) {
+                r[k] = __uint_as_float(0xffc00000u);
+            }
+        }
         float uv[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
         const bool has_uv = seg.uv_off != kB2Invalid;
         if (has_uv) {

@@ -72,6 +72,27 @@ uint64_t crt_hostcheck_digest(void *p)
     return d;
 }
 
+// The host-built scene as set_scene uploads it (sizes from crt_hostcheck_stats): nodes (80 B per node), tri_order (leaf
+// order -> flattened triangle), packed triangles (12 floats per triangle) and shading records (48 B per triangle), both
+// in leaf order. Any pointer may be null.
+void crt_hostcheck_export(void *p, void *nodes, uint32_t *tri_order, float *tris, void *shade)
+{
+    const HostCheck *h = static_cast<const HostCheck *>(p);
+    const size_t n = h->rec.bvh.tri_order.size();
+    if (nodes) {
+        std::memcpy(nodes, h->rec.bvh.nodes.data(), h->rec.bvh.nodes.size() * sizeof(crt::Bvh8Node));
+    }
+    if (tri_order && n) {
+        std::memcpy(tri_order, h->rec.bvh.tri_order.data(), n * sizeof(uint32_t));
+    }
+    if (tris && n) {
+        std::memcpy(tris, h->rec.tris.data(), n * 12 * sizeof(float));
+    }
+    if (shade && n) {
+        std::memcpy(shade, h->rec.shade.data(), n * sizeof(crt::TriShade));
+    }
+}
+
 // rays: n*8 floats; hits: n*4 floats {t,u,v,bits(flat id)}; normals (optional) n*3;
 // counters (optional) n*2 uint32 {nodes visited, triangles tested}
 void crt_hostcheck_trace(void *p, const float *rays, uint64_t n, int any_hit, float *hits, float *normals,

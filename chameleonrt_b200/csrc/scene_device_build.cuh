@@ -46,6 +46,20 @@ struct EventSet {
     cudaEvent_t operator[](size_t i) const { return ev[i]; }
 };
 
+// The binary tree behind a device build, copied out before its buffers are released (bvh_devcheck.cu; the renderer
+// leaves DeviceSceneBuild::dump null): the sorted Morton keys and triangle ids, the centroid bounds (ordered uints),
+// and per BVH2 node id (bvh8_device.cuh: Lbvh) the children, boxes, costs and decisions.
+struct Bvh2Dump {
+    std::vector<crt::u64> keys;
+    std::vector<uint32_t> vals;
+    uint32_t cbounds[6] = {0, 0, 0, 0, 0, 0};
+    std::vector<uint2> children;         // n - 1
+    std::vector<float4> box_lo, box_hi;  // 2n - 1
+    std::vector<float> cost;             // 7 (2n - 1)
+    std::vector<uint8_t> decision;       // 7 (2n - 1)
+    uint32_t root = 0;
+};
+
 struct DeviceSceneBuild {
     // in
     cudaStream_t stream = nullptr;
@@ -60,6 +74,7 @@ struct DeviceSceneBuild {
     int rounds = 0;                        // PLOC rounds
     double build_ms = 0.0;                 // CUDA events around everything after the flattening
     double phase_ms[5] = {0, 0, 0, 0, 0};  // flatten (host wall clock), keys + sort, binary tree, BVH8 emission, packing
+    Bvh2Dump *dump = nullptr;              // when set (the test-only check library): the intermediate state of the build
 
     void run(const crt_scene_t *scene, const crt::FlattenPlan &plan)
     {
@@ -83,6 +98,25 @@ struct DeviceSceneBuild {
             crt::k_scan_add<T><<<tiles, crt::kBuildBlock, 0, stream>>>(out, n, scratch);
         }
     }
+    // Stable LSD radix sort of n (key, value) pairs by the whole 64-bit key (Morton keys use 63 bits): 8 passes of
+    // 8 bits, k_radix_hist -> scan of the digit-major histogram -> k_radix_scatter. The pairs end where they started
+    // (an even number of passes); keys_tmp / vals_tmp hold every other pass. hist: 256 per tile of n; scratch:
+    // scan_scratch_items(256 * tiles).
+    void radix_sort(crt::u64 *keys, uint32_t *vals, crt::u64 *keys_tmp, uint32_t *vals_tmp, uint32_t n, uint32_t *hist,
+                    uint32_t *scratch)
+    {
+        const uint32_t tiles = (n + crt::kBuildTile - 1) / crt::kBuildTile;
+        crt::u64 *kin = keys, *kout = keys_tmp;
+        uint32_t *vin = vals, *vout = vals_tmp;
+        for (int shift = 0; shift < 64; shift += 8) {  // 63 key bits
+            crt::k_radix_hist<<<tiles, crt::kBuildBlock, 0, stream>>>(kin, n, shift, hist, tiles);
+            device_scan<uint32_t>(hist, hist, tiles * 256u, scratch);
+            crt::k_radix_scatter<<<tiles, crt::kBuildBlock, 0, stream>>>(kin, vin, kout, vout, n, shift, hist, tiles);
+            std::swap(kin, kout);
+            std::swap(vin, vout);
+        }
+    }
+
     static size_t scan_scratch_items(size_t n)
     {
         size_t total = 0;
@@ -272,15 +306,9 @@ struct DeviceSceneBuild {
         const unsigned g = grid_for(n);
         crt::k_lbvh_bounds<<<g, crt::kBuildBlock, 0, stream>>>(b);
         crt::k_lbvh_keys<<<g, crt::kBuildBlock, 0, stream>>>(b, keys0.ptr, vals0.ptr);
-        crt::u64 *kin = keys0.ptr, *kout = keys1.ptr;
-        uint32_t *vin = vals0.ptr, *vout = vals1.ptr;
-        for (int shift = 0; shift < 64; shift += 8) {  // 63 key bits
-            crt::k_radix_hist<<<tiles, crt::kBuildBlock, 0, stream>>>(kin, n, shift, hist.ptr, tiles);
-            device_scan<uint32_t>(hist.ptr, hist.ptr, tiles * 256u, reinterpret_cast<uint32_t *>(scan_scratch.ptr));
-            crt::k_radix_scatter<<<tiles, crt::kBuildBlock, 0, stream>>>(kin, vin, kout, vout, n, shift, hist.ptr, tiles);
-            std::swap(kin, kout);
-            std::swap(vin, vout);
-        }
+        radix_sort(keys0.ptr, vals0.ptr, keys1.ptr, vals1.ptr, n, hist.ptr, reinterpret_cast<uint32_t *>(scan_scratch.ptr));
+        crt::u64 *const kin = keys0.ptr;  // (eight passes: the sorted pairs are back in keys0 / vals0)
+        uint32_t *const vin = vals0.ptr;
         CUDA_CHECK(cudaEventRecord(ev_sorted, stream));
         crt::u64 *h_tail = nullptr;  // pinned: last offset + last count of a scan = its total
         CUDA_CHECK(cudaMallocHost(&h_tail, 2 * sizeof(crt::u64)));
@@ -401,6 +429,21 @@ struct DeviceSceneBuild {
         CUDA_CHECK(cudaGetLastError());
         std::vector<uint32_t> order(n);
         CUDA_CHECK(cudaMemcpyAsync(order.data(), tri_order.ptr, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+        if (dump) {
+            auto fetch = [&](auto &dst, const auto *src, size_t count) {
+                dst.resize(count);
+                CUDA_CHECK(cudaMemcpyAsync(dst.data(), src, count * sizeof(*src), cudaMemcpyDeviceToHost, stream));
+            };
+            fetch(dump->keys, kin, n);
+            fetch(dump->vals, vin, n);
+            fetch(dump->children, d_children.ptr, n - 1);
+            fetch(dump->box_lo, box_lo.ptr, num_b2);
+            fetch(dump->box_hi, box_hi.ptr, num_b2);
+            fetch(dump->cost, cost.ptr, (size_t)num_b2 * 7);
+            fetch(dump->decision, decision.ptr, (size_t)num_b2 * 7);
+            CUDA_CHECK(cudaMemcpyAsync(dump->cbounds, cbounds.ptr, sizeof(dump->cbounds), cudaMemcpyDeviceToHost, stream));
+            dump->root = root;
+        }
         CUDA_CHECK(cudaStreamSynchronize(stream));
         float t = 0.f;
         CUDA_CHECK(cudaEventElapsedTime(&t, ev0, ev1));

@@ -100,6 +100,7 @@ class HostCheck:
         lib.crt_hostcheck_last_error.restype = C.c_char_p
         lib.crt_hostcheck_digest.restype = C.c_uint64
         lib.crt_hostcheck_digest.argtypes = [C.c_void_p]
+        lib.crt_hostcheck_export.argtypes = [C.c_void_p] * 5
         self.lib = lib
         ms = scene.to_c()
         self.h = lib.crt_hostcheck_create(C.byref(ms.c), threads)
@@ -118,6 +119,17 @@ class HostCheck:
 
     def digest(self) -> int:
         return int(self.lib.crt_hostcheck_digest(self.h))
+
+    def export(self):
+        """The scene as set_scene uploads it: BVH8 nodes (uint8, 80 per node), tri_order (leaf order -> flattened
+        triangle), packed triangles (float32, 12 per triangle) and shading records (float32, 12 per triangle)."""
+        st = self.stats()
+        nodes = np.zeros((st["nodes"], 80), np.uint8)
+        order = np.zeros(st["tris"], np.uint32)
+        tris = np.zeros((st["tris"], 12), np.float32)
+        shade = np.zeros((st["tris"], 12), np.float32)
+        self.lib.crt_hostcheck_export(self.h, nodes.ctypes.data, order.ctypes.data, tris.ctypes.data, shade.ctypes.data)
+        return nodes, order, tris, shade
 
     def trace(self, rays, any_hit=False, normals=False, counters=False, far_first=False):
         rays = np.ascontiguousarray(rays, np.float32).reshape(-1, 8)

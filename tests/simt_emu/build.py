@@ -50,20 +50,50 @@ def build(force: bool = False) -> str:
     with open(gen, "w") as f:
         f.write('#include "simt_env.h"\n' + translate(open(os.path.join(CSRC, "crt_cuda_core.cu")).read().replace(
             '"../../include/crt_cuda.h"', f'"{ROOT}/include/crt_cuda.h"'), 21))
+    _write_driver()
+    _link(LIB, gen)
+    return LIB
+
+
+def _write_driver():
     # the device set_scene driver is a header of the same translation unit: its translated copy sits next to the
     # generated source, where the quoted include finds it first
     with open(os.path.join(OUT, "scene_device_build.cuh"), "w") as f:
         f.write(translate(open(os.path.join(CSRC, "scene_device_build.cuh")).read().replace(
             '"../../include/crt_scene.h"', f'"{ROOT}/include/crt_scene.h"'), 18))
+
+
+def _link(lib, gen):
     cuda_inc = os.path.join(os.path.dirname(os.path.dirname(os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc"))), "include")
     subprocess.check_call(["make", "-s", "-C", CSRC, "host_scene.o", "bvh8_build.o"])
     subprocess.check_call(["g++", "-std=c++17", "-O2", "-fPIC", "-pthread", "-march=x86-64-v3", "-ffp-contract=off", "-Wno-attributes",
                            "-I" + CSRC, "-I" + cuda_inc, "-shared",
                            # -Bsymbolic: the library's calls to cudaMalloc & co. must bind to ITS stubs even when a real
                            # libcudart is already in the process (torch loads one globally)
-                           "-Wl,-Bsymbolic", "-o", LIB, gen, os.path.join(HERE, "cuda_emu.cpp"),
+                           "-Wl,-Bsymbolic", "-o", lib, gen, os.path.join(HERE, "cuda_emu.cpp"),
                            os.path.join(CSRC, "host_scene.o"), os.path.join(CSRC, "bvh8_build.o")])
-    return LIB
+
+
+DEVCHECK_LIB = os.path.join(OUT, "libcrt_bvh_devcheck_simt.so")
+
+
+def build_bvh_devcheck(force: bool = False) -> str:
+    """_build/libcrt_bvh_devcheck_simt.so: chameleonrt_b200/csrc/bvh_devcheck.cu (which has no launch of its own)
+    compiled for the host next to the translated scene_device_build.cuh, with every kernel launch of the device build
+    under the SIMT environment (tests/test_bvh_build_exact.py)."""
+    srcs = [os.path.join(CSRC, f) for f in ("bvh_devcheck.cu", "scene_device_build.cuh", "cuda_host_utils.h", "bvh8_device.cuh", "bvh8_traverse.h", "simt_env.h",
+                                            "host_scene.h", "host_scene.cpp", "bvh8.h", "bvh8_build.cpp")] + [os.path.join(HERE, "cuda_emu.cpp"), __file__]
+    if not force and os.path.exists(DEVCHECK_LIB) and all(os.path.getmtime(DEVCHECK_LIB) >= os.path.getmtime(s) for s in srcs):
+        return DEVCHECK_LIB
+    os.makedirs(OUT, exist_ok=True)
+    gen = os.path.join(OUT, "bvh_devcheck_simt.cpp")
+    src = open(os.path.join(CSRC, "bvh_devcheck.cu")).read()
+    assert "<<<" not in src, "bvh_devcheck.cu must not launch kernels itself"
+    with open(gen, "w") as f:
+        f.write('#include "simt_env.h"\n' + src.replace('"../../include/crt_scene.h"', f'"{ROOT}/include/crt_scene.h"'))
+    _write_driver()
+    _link(DEVCHECK_LIB, gen)
+    return DEVCHECK_LIB
 
 
 def build_plugin(force: bool = False):
@@ -92,4 +122,5 @@ def build_plugin(force: bool = False):
 
 if __name__ == "__main__":
     print(build(force=True))
+    print(build_bvh_devcheck(force=True))
     print(build_plugin(force=True))
