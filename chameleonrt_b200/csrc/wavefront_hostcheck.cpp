@@ -263,6 +263,54 @@ struct HostWavefront {
     }
 };
 
+// wave_devcheck.cu's state image, layout and view arguments as the kernels' structs (host pointers, used in place)
+crt::PathState state_image(void *const *st)
+{
+    static unsigned long long trav[4];
+    auto f4 = [&](int k) { return static_cast<float4 *>(st[k]); };
+    crt::PathState ps;
+    ps.ray_o = f4(0);
+    ps.ray_d = f4(1);
+    ps.hit = f4(2);
+    ps.thr_rng = f4(3);
+    ps.radiance = f4(4);
+    ps.nee_T = f4(5);
+    ps.nee_l1 = f4(6);
+    ps.nee_l2 = f4(7);
+    ps.sray_o = f4(8);
+    ps.sray_d = f4(9);
+    ps.vis = static_cast<uint8_t *>(st[10]);
+    ps.queue[0] = static_cast<uint32_t *>(st[11]);
+    ps.queue[1] = static_cast<uint32_t *>(st[12]);
+    ps.counters = static_cast<uint32_t *>(st[13]);
+    ps.trav_counters = trav;
+    return ps;
+}
+
+crt::FrameLayout frame_layout(const uint32_t *lay, const uint32_t *tile_ids)
+{
+    crt::FrameLayout fl;
+    fl.fb_w = (int)lay[0];
+    fl.fb_h = (int)lay[1];
+    fl.ntx = lay[2];
+    fl.npx_local = lay[3];
+    fl.spp = lay[4];
+    fl.frames = lay[5];
+    fl.tile_ids = tile_ids;
+    return fl;
+}
+
+crt::ViewParams view_params(const float *v, uint32_t frame_id)
+{
+    crt::ViewParams view;
+    view.pos = make_float3(v[0], v[1], v[2]);
+    view.dir_du = make_float3(v[3], v[4], v[5]);
+    view.dir_dv = make_float3(v[6], v[7], v[8]);
+    view.dir_top_left = make_float3(v[9], v[10], v[11]);
+    view.frame_id = frame_id;
+    return view;
+}
+
 }  // namespace
 
 extern "C" {
@@ -321,5 +369,132 @@ void crt_wavecheck_read(void *p, float *accum_full, uint32_t *img_full)
     HostWavefront *r = static_cast<HostWavefront *>(p);
     std::memcpy(accum_full, r->accum_full.data(), r->accum_full.size() * sizeof(float));
     std::memcpy(img_full, r->img_full.data(), r->img_full.size() * sizeof(uint32_t));
+}
+
+// ---- the per-stage entry points of wave_devcheck.cu (same names, signatures and state image), over the one-lane
+// launches above: tests/test_wavefront_device.py runs each stage here on the state it gave the device ----
+
+const char *wavekat_last_error() { return g_err.c_str(); }
+
+void *wavekat_scene(const crt_scene_t *scene)
+{
+    try {
+        auto *r = new HostWavefront();
+        r->set_scene(scene);
+        return r;
+    } catch (const std::exception &e) {
+        g_err = e.what();
+        return nullptr;
+    }
+}
+
+void wavekat_scene_free(void *s) { delete static_cast<HostWavefront *>(s); }
+
+// (this build only) the scene's records as both builds upload them, for the restatements: field 0 shading records
+// (48 B per triangle, leaf order), 1 materials (64 B each), 2 lights (80 B each), 3 texel arena (4 B per texel),
+// 4 texture descriptors (16 B each). dst null: only the size. Returns the bytes, -1 for an unknown field.
+long long wavekat_records(void *scene, int field, void *dst)
+{
+    const crt::SceneRecords &rec = static_cast<HostWavefront *>(scene)->rec;
+    auto put = [&](const auto &v) {
+        const size_t bytes = v.size() * sizeof(v[0]);
+        if (dst && bytes) {
+            std::memcpy(dst, v.data(), bytes);
+        }
+        return (long long)bytes;
+    };
+    switch (field) {
+    case 0: return put(rec.shade);
+    case 1: return put(rec.shading.materials);
+    case 2: return put(rec.shading.lights);
+    case 3: return put(rec.shading.texels);
+    case 4: return put(rec.shading.tex_desc);
+    default: return -1;
+    }
+}
+
+int wavekat_raygen(const float *view, uint32_t frame_id, const uint32_t *lay, const uint32_t *tile_ids, const uint32_t *sel,
+                   uint32_t cap, void *const *st)
+{
+    const crt::PathState ps = state_image(st);
+    const crt::FrameLayout fl = frame_layout(lay, tile_ids);
+    const crt::ViewParams v = view_params(view, frame_id);
+    const size_t npaths = (size_t)fl.npx_local * fl.spp * fl.frames;
+    (void)cap;
+    if (sel) {
+        crt::AdaptiveFrame ad{};
+        ad.sel = reinterpret_cast<const uint2 *>(sel);
+        HostWavefront::launch(npaths, [&] { crt::k_raygen<true>(v, fl, ps, ad); });
+    } else {
+        HostWavefront::launch(npaths, [&] { crt::k_raygen<false>(v, fl, ps); });
+    }
+    return 0;
+}
+
+int wavekat_traverse(void *scene, int queue_index, int closest_counter, int any_counter, int work_counter, int far_first,
+                     uint32_t cap, void *const *st)
+{
+    HostWavefront *r = static_cast<HostWavefront *>(scene);
+    const crt::PathState ps = state_image(st);
+    (void)work_counter;
+    (void)cap;
+    r->traverse(ps, ps.queue[queue_index & 1], closest_counter >= 0 ? ps.counters[closest_counter] : 0u,
+                any_counter >= 0 ? ps.counters[any_counter] : 0u, far_first != 0);
+    return 0;
+}
+
+int wavekat_shade(void *scene, int bounce, int max_depth, uint32_t cap, void *const *st)
+{
+    const crt::DeviceScene sc = static_cast<HostWavefront *>(scene)->device_scene();
+    const crt::PathState ps = state_image(st);
+    HostWavefront::launch(cap, [&] { crt::k_shade<false>(sc, ps, ps.queue[bounce & 1], ps.queue[(bounce + 1) & 1], bounce, max_depth); });
+    return 0;
+}
+
+int wavekat_nee_resolve(int bounce, uint32_t cap, void *const *st, uint32_t *grid)
+{
+    const crt::PathState ps = state_image(st);
+    *grid = cap;
+    HostWavefront::launch(cap, [&] { crt::k_nee_resolve(ps, ps.queue[bounce & 1], bounce); });
+    return 0;
+}
+
+int wavekat_resolve(const uint32_t *lay, const uint32_t *tile_ids, uint32_t frame_id, const uint32_t *sel, float *moments,
+                    uint32_t stat_base, float *accum_local, uint32_t *img_local, float *accum_full, uint32_t *img_full,
+                    uint32_t cap, void *const *st)
+{
+    const crt::PathState ps = state_image(st);
+    const crt::FrameLayout fl = frame_layout(lay, tile_ids);
+    (void)cap;
+    if (sel) {
+        crt::AdaptiveFrame ad{};
+        ad.sel = reinterpret_cast<const uint2 *>(sel);
+        ad.moments = reinterpret_cast<float2 *>(moments);
+        ad.stat_base = stat_base;
+        HostWavefront::launch(fl.npx_local, [&] {
+            crt::k_resolve<true>(fl, ps, frame_id, accum_local, img_local, accum_full, img_full, nullptr, nullptr, 0u, ad);
+        });
+    } else {
+        HostWavefront::launch(fl.npx_local, [&] {
+            crt::k_resolve<false>(fl, ps, frame_id, accum_local, img_local, accum_full, img_full, nullptr, nullptr, 0u);
+        });
+    }
+    return 0;
+}
+
+// the shade-queue sort's result: a stable sort of the queue by shade_bucket (k_queue_hist / k_queue_scatter need a
+// 256-thread block, which this build does not have)
+int wavekat_queue_sort(void *scene, int bounce, uint32_t cap, void *const *st, uint32_t *sorted)
+{
+    const crt::DeviceScene sc = static_cast<HostWavefront *>(scene)->device_scene();
+    const crt::PathState ps = state_image(st);
+    (void)cap;
+    const uint32_t *qin = ps.queue[bounce & 1];
+    const uint32_t n = ps.counters[crt::kCntQueue + bounce];
+    std::vector<uint32_t> q(qin, qin + n);
+    std::stable_sort(q.begin(), q.end(),
+                     [&](uint32_t a, uint32_t b) { return crt::shade_bucket(sc, ps, a) < crt::shade_bucket(sc, ps, b); });
+    std::copy(q.begin(), q.end(), sorted);
+    return 0;
 }
 }
