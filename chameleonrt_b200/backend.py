@@ -18,7 +18,7 @@ from typing import Optional
 
 import numpy as np
 
-from .scene import CRenderStats, CScene, RenderStats, Scene
+from .scene import CQuadLight, CRenderStats, CScene, RenderStats, Scene
 
 _CSRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "csrc")
 _LIB_PATH = os.path.join(_CSRC, "libcrt_cuda_core.so")
@@ -37,6 +37,7 @@ C_ABI_SYMBOLS = (
     "crtc_get_counters", "crtc_get_scene_info", "crtc_trace_closest", "crtc_trace_any", "crtc_bench_trace",
     "crtc_local_buffers", "crtc_assemble_rank", "crtc_export_frame", "crtc_import_frame", "crtc_share_frame", "crtc_read_img", "crtc_frame_wait", "crtc_copy_img_to_array",
     "crtc_read_aov", "crtc_denoise", "crtc_read_denoise_history", "crtc_set_adaptive", "crtc_read_adaptive",
+    "crtc_update_instances", "crtc_update_vertices", "crtc_update_lights", "crtc_commit_scene",
 )
 # Per-pixel layout of crtc_read_aov: name -> (first float, number of floats)
 AOV_LAYOUT = {"albedo": (0, 3), "coverage": (3, 1), "normal": (4, 3), "depth": (7, 1), "lum_m1": (8, 1), "lum_m2": (9, 1)}
@@ -105,6 +106,10 @@ def load_lib() -> C.CDLL:
     lib.crtc_read_denoise_history.argtypes = [vp, vp]
     lib.crtc_set_adaptive.argtypes = [vp, C.POINTER(CAdaptiveParams)]
     lib.crtc_read_adaptive.argtypes = [vp, vp, vp]
+    lib.crtc_update_instances.argtypes = [vp, C.c_uint32, C.c_uint32, vp]
+    lib.crtc_update_vertices.argtypes = [vp, C.c_uint32, C.c_uint32, vp, C.c_uint32]
+    lib.crtc_update_lights.argtypes = [vp, vp, C.c_uint32]
+    lib.crtc_commit_scene.argtypes = [vp]
     _lib = lib
     return lib
 
@@ -121,7 +126,7 @@ class RenderCUDA:
                  count_traversal: bool = False, bvh_threads: int = 0, stream: Optional[int] = None,
                  any_far_first: Optional[int] = None, bvh_builder: Optional[str] = None,
                  tri_pass_defer: Optional[int] = None, shade_sort: Optional[int] = None, aov: bool = False,
-                 denoise_history: int = 0):
+                 denoise_history: int = 0, dynamic_scene: bool = False):
         self.lib = load_lib()
         self.h = C.c_void_p()
         self._check(self.lib.crtc_create(C.byref(self.h), device))
@@ -161,6 +166,8 @@ class RenderCUDA:
             self._check(self.lib.crtc_set_option(self.h, b"aov", 1))
         if denoise_history:  # denoise() carries a reprojected history of up to this many samples (option "denoise_history")
             self._check(self.lib.crtc_set_option(self.h, b"denoise_history", int(denoise_history)))
+        if dynamic_scene:  # set_scene keeps what update_instances / update_vertices + commit_scene need (option "dynamic_scene")
+            self._check(self.lib.crtc_set_option(self.h, b"dynamic_scene", 1))
         if stream is not None:
             self._check(self.lib.crtc_set_stream(self.h, C.c_void_p(stream)))
         self.width = self.height = 0
@@ -199,6 +206,34 @@ class RenderCUDA:
         c_scene.contents.samples_per_pixel = samples_per_pixel
         self.samples_per_pixel = samples_per_pixel
         self._check(self.lib.crtc_set_scene(self.h, c_scene))
+
+    # ---- scene updates between frames (include/crt_cuda.h: crtc_update_instances ... crtc_commit_scene) ----
+    def update_instances(self, transforms, first: int = 0) -> None:
+        """Stages new object_to_world matrices for instances ``first`` .. ``first + n - 1``: (n, 4, 4) or (n, 16) in
+        ``Instance.transform``'s layout (row i, column j). Needs ``dynamic_scene=True`` at the last set_scene."""
+        m = np.asarray(transforms, dtype=np.float32).reshape(-1, 4, 4)
+        col_major = np.ascontiguousarray(m.transpose(0, 2, 1))  # crt_instance_t::transform
+        self._check(self.lib.crtc_update_instances(self.h, int(first), m.shape[0], col_major.ctypes.data))
+
+    def update_vertices(self, mesh: int, geometry: int, vertices) -> None:
+        """Stages new object-space positions (n, 3) for geometry ``geometry`` of mesh ``mesh``; n must be its vertex
+        count at set_scene. Needs ``dynamic_scene=True`` at the last set_scene."""
+        v = np.ascontiguousarray(vertices, dtype=np.float32).reshape(-1, 3)
+        self._check(self.lib.crtc_update_vertices(self.h, int(mesh), int(geometry), v.ctypes.data if len(v) else None,
+                                                  v.shape[0]))
+
+    def update_lights(self, lights) -> None:
+        """Stages a new list of ``QuadLight``s (the count may change)."""
+        arr = (CQuadLight * max(1, len(lights)))()
+        for i, l in enumerate(lights):
+            raw = np.array(l.as_floats(), dtype=np.float32)
+            C.memmove(C.addressof(arr[i]), raw.ctypes.data, 80)
+        self._check(self.lib.crtc_update_lights(self.h, C.addressof(arr), len(lights)))
+
+    def commit_scene(self) -> None:
+        """Applies the staged updates on the renderer's stream: later frames see the updated scene, from a reset
+        accumulation. Nothing staged: nothing happens."""
+        self._check(self.lib.crtc_commit_scene(self.h))
 
     def render(self, pos, dir, up, fovy: float, camera_changed: bool, readback_framebuffer: bool = True) -> RenderStats:
         _p, pp = _vec3(pos)

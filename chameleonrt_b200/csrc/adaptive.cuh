@@ -9,7 +9,7 @@
 // frame_id and folds the luminance moments (kernels.cuh). A pixel that is not enqueued costs no traversal or shading work:
 // every later kernel reads its ray count from the device counters. The definitions are in include/crt_cuda.h.
 //
-// Kernels are launched through aov_launch (aov_denoise.cuh), so the host build of the renderer (tests/simt_emu) compiles
+// Kernels are launched through crt_host::launch (cuda_host_utils.h), so the host build of the renderer (tests/simt_emu) compiles
 // this header unchanged.
 #pragma once
 
@@ -124,19 +124,19 @@ struct AdaptiveState {
     AdaptiveFrame frame(uint32_t stat_base) const { return AdaptiveFrame{sel.ptr, moments.ptr, stat_base}; }
     void select(const FrameLayout &f, const AdaptiveSelect &p, cudaStream_t stream)
     {
-        aov_launch(k_adaptive_select, f.npx_local / kAdaptiveBlock, kAdaptiveBlock, stream, f, p, count.ptr, sel.ptr, moments.ptr);
+        crt_host::launch(k_adaptive_select, f.npx_local / kAdaptiveBlock, kAdaptiveBlock, stream, f, p, count.ptr, sel.ptr, moments.ptr);
     }
     // The adaptive instantiations of the frame's first and last kernels (the mode-off ones are launched by the renderer)
     void raygen(unsigned grid, const ViewParams &view, const FrameLayout &f, const PathState &ps, const AdaptiveFrame &ad,
                 cudaStream_t stream)
     {
-        aov_launch(k_raygen<true>, grid, 256, stream, view, f, ps, ad);
+        crt_host::launch(k_raygen<true>, grid, 256, stream, view, f, ps, ad);
     }
     void resolve(unsigned grid, const FrameLayout &f, const PathState &ps, uint32_t frame_id, float *accum_local,
                  uint32_t *img_local, float *accum_full, uint32_t *img_full, uint32_t *done_counter, uint32_t *arrive_word,
                  uint32_t seq, const AdaptiveFrame &ad, cudaStream_t stream)
     {
-        aov_launch(k_resolve<true>, grid, 256, stream, f, ps, frame_id, accum_local, img_local, accum_full, img_full,
+        crt_host::launch(k_resolve<true>, grid, 256, stream, f, ps, frame_id, accum_local, img_local, accum_full, img_full,
                    done_counter, arrive_word, seq, ad);
     }
     // host arrays in, the local pixels' values over them, host arrays out (the other ranks' pixels stay as they were)
@@ -151,7 +151,7 @@ struct AdaptiveState {
             error_full.alloc(n);
             CUDA_CHECK(cudaMemcpyAsync(error_full.ptr, error_out, n * sizeof(float), cudaMemcpyHostToDevice, stream));
         }
-        aov_launch(k_adaptive_readout, (f.npx_local + 255) / 256, 256, stream, f, count.ptr, moments.ptr, stat_base,
+        crt_host::launch(k_adaptive_readout, (f.npx_local + 255) / 256, 256, stream, f, count.ptr, moments.ptr, stat_base,
                    samples_out ? samples_full.ptr : nullptr, error_out ? error_full.ptr : nullptr);
         if (samples_out) {
             CUDA_CHECK(cudaMemcpyAsync(samples_out, samples_full.ptr, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));

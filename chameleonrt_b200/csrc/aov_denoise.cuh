@@ -12,8 +12,8 @@
 // copy (the running mean's state) and a full row-major copy. The AOV kernels read only the path state and the scene and
 // write only these buffers, so a frame renders exactly the same with and without them.
 //
-// Every kernel is launched through aov_launch: chevrons under nvcc, simt::launch in the host build of the renderer
-// (tests/simt_emu), which compiles this header unchanged. Grids are one-dimensional for the same reason.
+// Every kernel is launched through crt_host::launch (cuda_host_utils.h), so that the host build of the renderer
+// (tests/simt_emu) compiles this header unchanged. Grids are one-dimensional for the same reason.
 #pragma once
 
 #include <cstdint>
@@ -27,20 +27,6 @@ namespace crt {
 constexpr int kAovFloats = 10;
 constexpr int kAovAlbedo = 0, kAovCoverage = 3, kAovNormal = 4, kAovDepth = 7, kAovLumM1 = 8, kAovLumM2 = 9;
 constexpr int kDenoiseBlock = 256;
-
-template <typename... P, typename... A>
-inline void aov_launch(void (*kernel)(P...), unsigned grid, unsigned block, cudaStream_t stream, A... args)
-{
-    if (grid == 0) {
-        return;
-    }
-#ifdef __CUDACC__
-    kernel<<<grid, block, 0, stream>>>(args...);
-#else
-    (void)stream;
-    simt::launch(grid, block, [&] { kernel(args...); });
-#endif
-}
 
 // One thread per local pixel; the batch's frames * spp samples in sample order, with k_resolve's slot indexing.
 // Hit: base colour as k_shade unpacks it (same template branch), the TriShade normal face-forwarded as k_shade does
@@ -506,14 +492,14 @@ struct AovState {
     {
         const unsigned g = (f.npx_local + 127) / 128;
         if (sc.tex_objects) {
-            aov_launch(k_aov_primary<true>, g, 128, stream, sc, f, ps, frame_id, local.ptr, full.ptr);
+            crt_host::launch(k_aov_primary<true>, g, 128, stream, sc, f, ps, frame_id, local.ptr, full.ptr);
         } else {
-            aov_launch(k_aov_primary<false>, g, 128, stream, sc, f, ps, frame_id, local.ptr, full.ptr);
+            crt_host::launch(k_aov_primary<false>, g, 128, stream, sc, f, ps, frame_id, local.ptr, full.ptr);
         }
     }
     void launch_moments(const FrameLayout &f, const PathState &ps, uint32_t frame_id, cudaStream_t stream)
     {
-        aov_launch(k_aov_moments, (f.npx_local + 255) / 256, 256, stream, f, ps, frame_id, local.ptr, full.ptr);
+        crt_host::launch(k_aov_moments, (f.npx_local + 255) / 256, 256, stream, f, ps, frame_id, local.ptr, full.ptr);
     }
     // Denoises the full frame `accum` (w x h x 3, `samples` = spp * frames accumulated) into dn_rgb / dn_img.
     // max_history > 0 (option denoise_history): the temporal pass runs between k_dn_prepare and the a-trous chain, with
@@ -538,7 +524,7 @@ struct AovState {
             }
         }
         const unsigned g = (unsigned)((n + kDenoiseBlock - 1) / kDenoiseBlock);
-        aov_launch(k_dn_prepare, g, kDenoiseBlock, stream, w, h, samples, accum, (const float *)full.ptr, dn_iv[0].ptr,
+        crt_host::launch(k_dn_prepare, g, kDenoiseBlock, stream, w, h, samples, accum, (const float *)full.ptr, dn_iv[0].ptr,
                    dn_guide.ptr, dn_grad.ptr);
         if (max_history) {
             if (hist_tag[hist_cur].valid && hist_tag[hist_cur].epoch < epoch) {
@@ -547,10 +533,10 @@ struct AovState {
             const HistoryTag &pt = hist_tag[hist_cur ^ 1];
             HistoryView pv{};
             const bool have_prev = pt.valid && pt.epoch < epoch && history_view(pt.view, pv);
-            aov_launch(k_dn_temporal, g, kDenoiseBlock, stream, w, h, samples, (float)max_history, view, pv,
+            crt_host::launch(k_dn_temporal, g, kDenoiseBlock, stream, w, h, samples, (float)max_history, view, pv,
                        have_prev ? (const float *)hist[hist_cur ^ 1].ptr : nullptr, (const float *)full.ptr,
                        (const float4 *)dn_guide.ptr, dn_iv[0].ptr, hist[hist_cur].ptr);
-            aov_launch(k_dn_variance, g, kDenoiseBlock, stream, w, h, prm.sigma_n, prm.sigma_z, (const float *)hist[hist_cur].ptr,
+            crt_host::launch(k_dn_variance, g, kDenoiseBlock, stream, w, h, prm.sigma_n, prm.sigma_z, (const float *)hist[hist_cur].ptr,
                        (const float4 *)dn_guide.ptr, (const float2 *)dn_grad.ptr, dn_iv[0].ptr);
             hist_tag[hist_cur].valid = true;
             hist_tag[hist_cur].epoch = epoch;
@@ -560,11 +546,11 @@ struct AovState {
             const float4 *in = dn_iv[i & 1].ptr;
             float4 *out = dn_iv[(i + 1) & 1].ptr;
             if (i + 1 == prm.iterations) {
-                aov_launch(k_dn_atrous<true>, g, kDenoiseBlock, stream, w, h, 1 << i, prm.sigma_l, prm.sigma_n, prm.sigma_z, in,
+                crt_host::launch(k_dn_atrous<true>, g, kDenoiseBlock, stream, w, h, 1 << i, prm.sigma_l, prm.sigma_n, prm.sigma_z, in,
                            out, (const float4 *)dn_guide.ptr, (const float2 *)dn_grad.ptr, (const float *)full.ptr, dn_rgb.ptr,
                            dn_img.ptr);
             } else {
-                aov_launch(k_dn_atrous<false>, g, kDenoiseBlock, stream, w, h, 1 << i, prm.sigma_l, prm.sigma_n, prm.sigma_z, in,
+                crt_host::launch(k_dn_atrous<false>, g, kDenoiseBlock, stream, w, h, 1 << i, prm.sigma_l, prm.sigma_n, prm.sigma_z, in,
                            out, (const float4 *)dn_guide.ptr, (const float2 *)dn_grad.ptr, (const float *)full.ptr, dn_rgb.ptr,
                            dn_img.ptr);
             }

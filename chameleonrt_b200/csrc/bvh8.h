@@ -45,6 +45,9 @@ static_assert(sizeof(Bvh8Node) == 80, "Bvh8Node must be 80 bytes (5 x 128-bit lo
 struct Bvh8 {
     std::vector<Bvh8Node> nodes;     // node 0 is the root
     std::vector<uint32_t> tri_order; // leaf order -> index of the input triangle
+    // the nodes are numbered level by level: level k is [level_begin[k], level_begin[k + 1]), the last entry is the
+    // node count (empty for a scene without triangles)
+    std::vector<uint32_t> level_begin;
     float scene_lo[3], scene_hi[3];
     // build statistics
     double sah_cost = 0.0;

@@ -841,6 +841,7 @@ void build_bvh8(const float *verts, size_t num_tris, int threads, Bvh8 &out)
     const auto t0 = std::chrono::steady_clock::now();
     out.nodes.clear();
     out.tri_order.clear();
+    out.level_begin.clear();
     out.max_depth = 0;
     if (threads <= 0) {
         threads = std::max(1u, std::thread::hardware_concurrency());
@@ -891,6 +892,7 @@ void build_bvh8(const float *verts, size_t num_tris, int threads, Bvh8 &out)
     size_t level_begin = 0, level_end = 1;
     while (level_begin < level_end) {
         ++out.max_depth;
+        out.level_begin.push_back((uint32_t)level_begin);
         const uint32_t kPlanBlock = 256;
         const uint32_t nb = (uint32_t)((level_end - level_begin + kPlanBlock - 1) / kPlanBlock);
         parallel_blocks(nb, threads, [&](uint32_t b) {
@@ -930,6 +932,7 @@ void build_bvh8(const float *verts, size_t num_tris, int threads, Bvh8 &out)
         level_begin = level_end;
         level_end = plans.size();
     }
+    out.level_begin.push_back((uint32_t)plans.size());
     lap("layout");
     // Fill pass (parallel): quantised child boxes, meta bytes and triangle order of every node.
     out.nodes.resize(plans.size());

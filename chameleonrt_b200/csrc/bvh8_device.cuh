@@ -78,78 +78,102 @@ __device__ __forceinline__ void dev_normalize3(float *v)
     v[2] *= c;
 }
 
+// The segment of flattened triangle f: the last one with flat_base <= f.
+__device__ __forceinline__ uint32_t dev_find_segment(const DevSegment *segs, uint32_t num_segs, uint32_t f)
+{
+    uint32_t lo = 0u, hi = num_segs - 1u;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1u) >> 1;
+        if (segs[mid].flat_base <= f) {
+            lo = mid;
+        } else {
+            hi = mid - 1u;
+        }
+    }
+    return lo;
+}
+
+// Flattened triangle f of segment seg (k_flatten, k_reflatten of scene_update.cuh): w = its world-space vertices
+// (9 floats), shade = its TriShade record. Returns false, with nothing written, if a vertex index is out of range.
 // xforms: 32 floats per instance = object_to_world, world_to_object (column-major). Arithmetic and its order are
 // those of flatten_scene (compiled with -fmad=false here, -ffp-contract=off there), so that the records are the same
 // bits: world-space vertices, normalize(transpose(world_to_object) * normalize(cross(v1 - v0, v2 - v0)))
 // (render_embree.ispc:269,288-290), material id, the three uvs, the flattened primitive id.
+__device__ __forceinline__ bool dev_flatten_triangle(const DevSegment &seg, uint32_t f, const float *xforms,
+                                                     const float *vert_arena, const uint32_t *index_arena,
+                                                     const float *uv_arena, float *w, float4 *shade)
+{
+    const uint32_t p = f - seg.flat_base;
+    const uint32_t *ip = index_arena + 3 * (size_t)(seg.tri_off + p);
+    const uint32_t idx[3] = {ip[0], ip[1], ip[2]};
+    if (idx[0] >= seg.num_verts || idx[1] >= seg.num_verts || idx[2] >= seg.num_verts) {
+        return false;
+    }
+    const float *m = xforms + (size_t)seg.instance * 32, *w2o = m + 16;
+    float vo[3][3];
+    for (int k = 0; k < 3; ++k) {
+        const float *v = vert_arena + 3 * (size_t)(seg.vert_off + idx[k]);
+        vo[k][0] = v[0];
+        vo[k][1] = v[1];
+        vo[k][2] = v[2];
+        w[3 * k] = m[0] * v[0] + m[4] * v[1] + m[8] * v[2] + m[12];
+        w[3 * k + 1] = m[1] * v[0] + m[5] * v[1] + m[9] * v[2] + m[13];
+        w[3 * k + 2] = m[2] * v[0] + m[6] * v[1] + m[10] * v[2] + m[14];
+    }
+    const float e1[3] = {vo[1][0] - vo[0][0], vo[1][1] - vo[0][1], vo[1][2] - vo[0][2]};
+    const float e2[3] = {vo[2][0] - vo[0][0], vo[2][1] - vo[0][1], vo[2][2] - vo[0][2]};
+    float n[3] = {e1[1] * e2[2] - e1[2] * e2[1], e1[2] * e2[0] - e1[0] * e2[2], e1[0] * e2[1] - e1[1] * e2[0]};
+    dev_normalize3(n);
+    float r[3];
+    r[0] = w2o[0] * n[0] + w2o[1] * n[1] + w2o[2] * n[2];
+    r[1] = w2o[4] * n[0] + w2o[5] * n[1] + w2o[6] * n[2];
+    r[2] = w2o[8] * n[0] + w2o[9] * n[1] + w2o[10] * n[2];
+    dev_normalize3(r);
+    for (int k = 0; k < 3; ++k) {
+        // a zero-area triangle's normal is 0 * inf: store the NaN flatten_scene gets on x86 (0xffc00000), not the
+        // GPU's canonical 0x7fffffff, so that the records are the same bits on both paths
+        if (r[k] != r[k]) {
+            r[k] = __uint_as_float(0xffc00000u);
+        }
+    }
+    float uv[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    const bool has_uv = seg.uv_off != kB2Invalid;
+    if (has_uv) {
+        for (int k = 0; k < 3; ++k) {
+            const float *t = uv_arena + 2 * (size_t)(seg.uv_off + idx[k]);
+            uv[2 * k] = t[0];
+            uv[2 * k + 1] = t[1];
+        }
+    }
+    // TriShade (host_scene.h): {n.xyz, material}, {uv0, uv1}, {uv2, has_uv, flat id}
+    shade[0] = make_float4(r[0], r[1], r[2], __uint_as_float(seg.mat_id));
+    shade[1] = make_float4(uv[0], uv[1], uv[2], uv[3]);
+    shade[2] = make_float4(uv[4], uv[5], __uint_as_float(has_uv ? 1u : 0u), __uint_as_float(f));
+    return true;
+}
+
 __global__ void __launch_bounds__(kBuildBlock) k_flatten(const DevSegment *segs, uint32_t num_segs, const float *xforms,
                                                          const float *vert_arena, const uint32_t *index_arena,
                                                          const float *uv_arena, uint32_t total, float *verts_out,
                                                          float4 *shade_out, uint32_t *bad_index)
 {
     for (uint32_t f = blockIdx.x * blockDim.x + threadIdx.x; f < total; f += gridDim.x * blockDim.x) {
-        uint32_t lo = 0u, hi = num_segs - 1u;  // the last segment with flat_base <= f
-        while (lo < hi) {
-            const uint32_t mid = (lo + hi + 1u) >> 1;
-            if (segs[mid].flat_base <= f) {
-                lo = mid;
-            } else {
-                hi = mid - 1u;
-            }
-        }
-        const DevSegment seg = segs[lo];
-        const uint32_t p = f - seg.flat_base;
-        const uint32_t *ip = index_arena + 3 * (size_t)(seg.tri_off + p);
-        const uint32_t idx[3] = {ip[0], ip[1], ip[2]};
-        float *w = verts_out + (size_t)f * 9;
-        if (idx[0] >= seg.num_verts || idx[1] >= seg.num_verts || idx[2] >= seg.num_verts) {
+        const DevSegment seg = segs[dev_find_segment(segs, num_segs, f)];
+        float w[9];
+        float4 shade[3];
+        if (!dev_flatten_triangle(seg, f, xforms, vert_arena, index_arena, uv_arena, w, shade)) {
             *bad_index = 1u;  // reported by the host after the launch
             for (int k = 0; k < 9; ++k) {
                 w[k] = 0.f;
             }
-            shade_out[(size_t)f * 3] = shade_out[(size_t)f * 3 + 1] = shade_out[(size_t)f * 3 + 2] = make_float4(0.f, 0.f, 0.f, 0.f);
-            continue;
+            shade[0] = shade[1] = shade[2] = make_float4(0.f, 0.f, 0.f, 0.f);
         }
-        const float *m = xforms + (size_t)seg.instance * 32, *w2o = m + 16;
-        float vo[3][3];
+        for (int k = 0; k < 9; ++k) {
+            verts_out[(size_t)f * 9 + k] = w[k];
+        }
         for (int k = 0; k < 3; ++k) {
-            const float *v = vert_arena + 3 * (size_t)(seg.vert_off + idx[k]);
-            vo[k][0] = v[0];
-            vo[k][1] = v[1];
-            vo[k][2] = v[2];
-            w[3 * k] = m[0] * v[0] + m[4] * v[1] + m[8] * v[2] + m[12];
-            w[3 * k + 1] = m[1] * v[0] + m[5] * v[1] + m[9] * v[2] + m[13];
-            w[3 * k + 2] = m[2] * v[0] + m[6] * v[1] + m[10] * v[2] + m[14];
+            shade_out[(size_t)f * 3 + k] = shade[k];
         }
-        const float e1[3] = {vo[1][0] - vo[0][0], vo[1][1] - vo[0][1], vo[1][2] - vo[0][2]};
-        const float e2[3] = {vo[2][0] - vo[0][0], vo[2][1] - vo[0][1], vo[2][2] - vo[0][2]};
-        float n[3] = {e1[1] * e2[2] - e1[2] * e2[1], e1[2] * e2[0] - e1[0] * e2[2], e1[0] * e2[1] - e1[1] * e2[0]};
-        dev_normalize3(n);
-        float r[3];
-        r[0] = w2o[0] * n[0] + w2o[1] * n[1] + w2o[2] * n[2];
-        r[1] = w2o[4] * n[0] + w2o[5] * n[1] + w2o[6] * n[2];
-        r[2] = w2o[8] * n[0] + w2o[9] * n[1] + w2o[10] * n[2];
-        dev_normalize3(r);
-        for (int k = 0; k < 3; ++k) {
-            // a zero-area triangle's normal is 0 * inf: store the NaN flatten_scene gets on x86 (0xffc00000), not the
-            // GPU's canonical 0x7fffffff, so that the records are the same bits on both paths
-            if (r[k] != r[k]) {
-                r[k] = __uint_as_float(0xffc00000u);
-            }
-        }
-        float uv[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-        const bool has_uv = seg.uv_off != kB2Invalid;
-        if (has_uv) {
-            for (int k = 0; k < 3; ++k) {
-                const float *t = uv_arena + 2 * (size_t)(seg.uv_off + idx[k]);
-                uv[2 * k] = t[0];
-                uv[2 * k + 1] = t[1];
-            }
-        }
-        // TriShade (host_scene.h): {n.xyz, material}, {uv0, uv1}, {uv2, has_uv, flat id}
-        shade_out[(size_t)f * 3] = make_float4(r[0], r[1], r[2], __uint_as_float(seg.mat_id));
-        shade_out[(size_t)f * 3 + 1] = make_float4(uv[0], uv[1], uv[2], uv[3]);
-        shade_out[(size_t)f * 3 + 2] = make_float4(uv[4], uv[5], __uint_as_float(has_uv ? 1u : 0u), __uint_as_float(f));
     }
 }
 
@@ -850,6 +874,57 @@ __global__ void __launch_bounds__(kBuildBlock) k_plan_level(Lbvh b, LevelArgs lv
 
 __device__ __forceinline__ float pow2_biased(int e) { return __uint_as_float((uint32_t)e << 23); }
 
+// The quantisation frame of a BVH8 node over its box [blo, bhi] (fill_node of bvh8_build.cpp; k_emit_level, k_bvh8_refit
+// of scene_update.cuh): out.p = blo and the exponents out.e; step = the grid step per axis. Flat axes get a thin but
+// non-zero grid, and the far plane of the node must be representable: lo + 255 * 2^e >= hi.
+__device__ __forceinline__ void bvh8_node_frame(const float *blo, const float *bhi, Bvh8Node &out, double *step)
+{
+    float max_ext = 0.f;
+    for (int a = 0; a < 3; ++a) {
+        out.p[a] = blo[a];
+        max_ext = fmaxf(max_ext, bhi[a] - blo[a]);
+    }
+    for (int a = 0; a < 3; ++a) {
+        float ext = fmaxf(bhi[a] - blo[a], max_ext * (1.f / 65536.f));
+        ext = fmaxf(ext, 1e-30f);
+        int e = (int)ceil(log2((double)ext / 255.0));
+        e = min(max(e, -100), 100);
+        while (e < 100 && (double)blo[a] + 255.0 * ldexp(1.0, e) < (double)bhi[a]) {
+            ++e;
+        }
+        out.e[a] = (uint8_t)(e + 127);
+        step[a] = (double)pow2_biased(e + 127);
+    }
+}
+
+// A child box [l3, h3] on the node's grid (bvh8_node_frame): conservative, at least one cell thick.
+__device__ __forceinline__ void bvh8_quantise_child(const Bvh8Node &out, const double *step, const float *l3, const float *h3,
+                                                    uint8_t *qlo, uint8_t *qhi)
+{
+    for (int a = 0; a < 3; ++a) {
+        const double p = out.p[a], st = step[a];
+        int lo = (int)floor(((double)l3[a] - p) / st);
+        int hi = (int)ceil(((double)h3[a] - p) / st);
+        lo = min(max(lo, 0), 255);
+        hi = min(max(hi, 0), 255);
+        while (lo > 0 && p + lo * st > (double)l3[a]) {  // conservative: p + q*step is exact in double
+            --lo;
+        }
+        while (hi < 255 && p + hi * st < (double)h3[a]) {
+            ++hi;
+        }
+        if (hi <= lo) {  // give flat boxes one grid cell of thickness
+            if (hi < 255) {
+                hi = lo + 1;
+            } else {
+                lo = hi - 1;
+            }
+        }
+        qlo[a] = (uint8_t)lo;
+        qhi[a] = (uint8_t)hi;
+    }
+}
+
 __global__ void __launch_bounds__(kBuildBlock) k_emit_level(Lbvh b, LevelArgs lv, const uint32_t *vals)
 {
     for (uint32_t w = blockIdx.x * blockDim.x + threadIdx.x; w < lv.count; w += gridDim.x * blockDim.x) {
@@ -859,25 +934,8 @@ __global__ void __launch_bounds__(kBuildBlock) k_emit_level(Lbvh b, LevelArgs lv
         const float4 plo = b.box_lo[root], phi = b.box_hi[root];
         const float blo[3] = {plo.x, plo.y, plo.z}, bhi[3] = {phi.x, phi.y, phi.z};
         alignas(16) Bvh8Node out;
-        float max_ext = 0.f;
-        for (int a = 0; a < 3; ++a) {
-            out.p[a] = blo[a];
-            max_ext = fmaxf(max_ext, bhi[a] - blo[a]);
-        }
         double step[3];
-        for (int a = 0; a < 3; ++a) {
-            // the quantisation frame of fill_node (bvh8_build.cpp): flat axes get a thin but non-zero grid, and the far
-            // plane of the node must be representable: lo + 255 * 2^e >= hi
-            float ext = fmaxf(bhi[a] - blo[a], max_ext * (1.f / 65536.f));
-            ext = fmaxf(ext, 1e-30f);
-            int e = (int)ceil(log2((double)ext / 255.0));
-            e = min(max(e, -100), 100);
-            while (e < 100 && (double)blo[a] + 255.0 * ldexp(1.0, e) < (double)bhi[a]) {
-                ++e;
-            }
-            out.e[a] = (uint8_t)(e + 127);
-            step[a] = (double)pow2_biased(e + 127);
-        }
+        bvh8_node_frame(blo, bhi, out, step);
         out.imask = 0;
         out.child_base = lv.next_begin + child_first;
         out.tri_base = tri_base;
@@ -889,28 +947,7 @@ __global__ void __launch_bounds__(kBuildBlock) k_emit_level(Lbvh b, LevelArgs lv
             if (cn != kB2Invalid) {
                 const float4 clo = b.box_lo[cn], chi = b.box_hi[cn];
                 const float l3[3] = {clo.x, clo.y, clo.z}, h3[3] = {chi.x, chi.y, chi.z};
-                for (int a = 0; a < 3; ++a) {
-                    const double p = out.p[a], st = step[a];
-                    int lo = (int)floor(((double)l3[a] - p) / st);
-                    int hi = (int)ceil(((double)h3[a] - p) / st);
-                    lo = min(max(lo, 0), 255);
-                    hi = min(max(hi, 0), 255);
-                    while (lo > 0 && p + lo * st > (double)l3[a]) {  // conservative: p + q*step is exact in double
-                        --lo;
-                    }
-                    while (hi < 255 && p + hi * st < (double)h3[a]) {
-                        ++hi;
-                    }
-                    if (hi <= lo) {  // give flat boxes one grid cell of thickness
-                        if (hi < 255) {
-                            hi = lo + 1;
-                        } else {
-                            lo = hi - 1;
-                        }
-                    }
-                    qlo[a] = (uint8_t)lo;
-                    qhi[a] = (uint8_t)hi;
-                }
+                bvh8_quantise_child(out, step, l3, h3, qlo, qhi);
                 if (lbvh_leaf_child(b, cn)) {
                     // the <= 3 triangles under cn, left to right
                     uint32_t st[4], k = 0u;

@@ -23,6 +23,7 @@
 #include "host_scene.h"
 #include "kernels.cuh"
 #include "scene_device_build.cuh"
+#include "scene_update.cuh"
 
 namespace {
 
@@ -210,6 +211,12 @@ struct crtc_renderer {
     }
     uint32_t num_lights = 0;
     std::vector<uint32_t> leaf_flat_ids;  // host copy: leaf-order triangle -> flattened prim id
+    // Option "dynamic_scene" (scene_update.cuh): `dynamic_scene` is the option, `scene_update` what the last set_scene
+    // kept for updates (null with the option off). Lights need no kept state: `staged_lights` waits for the commit.
+    bool dynamic_scene = false;
+    std::unique_ptr<crt_host::SceneUpdate> scene_update;
+    std::vector<crt_quad_light_t> staged_lights;
+    bool lights_staged = false;
     double scene_info[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};  // crtc_get_scene_info
     double phase_ms[5] = {0, 0, 0, 0, 0};  // last set_scene: flatten, keys + sort, binary tree, BVH8 emission, packing
 
@@ -705,6 +712,9 @@ struct crtc_renderer {
     void set_scene(const crt_scene_t *scene)
     {
         make_current();
+        scene_update.reset();  // (drops staged updates too)
+        lights_staged = false;
+        staged_lights.clear();
         frame_id = 0;
         adaptive_epoch = false;
         auto_frames = 0;
@@ -717,8 +727,11 @@ struct crtc_renderer {
         crt::FlattenPlan plan;
         crt::plan_flatten(scene, plan);
         crt::check_triangle_count(plan.total_tris);
+        std::unique_ptr<crt_host::SceneUpdate> keep(dynamic_scene ? new crt_host::SceneUpdate() : nullptr);
+        std::vector<uint32_t> level_begin;
         bool built_on_device = false;
-        if (bvh_builder != 0 && plan.total_tris > 0) {
+        const bool try_device = bvh_builder != 0 && plan.total_tris > 0;
+        if (try_device) {
             // set_scene on the device: only the references are checked and the materials / textures converted on the host
             crt::pack_shading(scene, bvh_threads, rec.shading);
             crt_host::DeviceSceneBuild job;
@@ -731,6 +744,7 @@ struct crtc_renderer {
             job.d_tris = &d_tris;
             job.d_shade = &d_shade;
             job.leaf_flat_ids = &leaf_flat_ids;
+            job.geometry = keep ? keep->geometry.get() : nullptr;
             try {
                 job.run(scene, plan);
                 built_on_device = true;
@@ -746,6 +760,7 @@ struct crtc_renderer {
                 bvh_nodes = job.num_nodes;
                 bvh_depth = job.depth;
                 bvh_ms = job.build_ms;
+                level_begin = job.level_begin;
                 build_rounds = job.rounds;
                 for (int i = 0; i < 5; ++i) {
                     phase_ms[i] = job.phase_ms[i];
@@ -766,6 +781,13 @@ struct crtc_renderer {
             bvh_nodes = (uint32_t)rec.bvh.nodes.size();
             bvh_depth = rec.bvh.max_depth;
             bvh_ms = rec.bvh.build_seconds * 1e3;
+            level_begin = rec.bvh.level_begin;
+            if (keep && !try_device) {
+                keep->geometry->upload(scene, plan, stream);  // (a device build that fell back has uploaded it already)
+            }
+        }
+        if (keep) {
+            keep->keep(scene, leaf_flat_ids, level_begin, stream);
         }
         const crt::ShadingRecords &sh = rec.shading;
         static_assert(sizeof(crt_material_t) == 64 && sizeof(crt_quad_light_t) == 80, "layouts");
@@ -796,6 +818,61 @@ struct crtc_renderer {
             }
         }
         aov_state.drop_history();  // (a history of another scene does not reproject)
+        scene_update = std::move(keep);
+    }
+
+    // ---- scene updates (include/crt_cuda.h: crtc_update_instances ... crtc_commit_scene) ----
+    crt_host::SceneUpdate &require_dynamic(const char *what)
+    {
+        require_scene();
+        if (!scene_update) {
+            throw std::runtime_error(std::string(what) + ": needs option dynamic_scene = 1 at the last crtc_set_scene");
+        }
+        return *scene_update;
+    }
+    void update_lights(const crt_quad_light_t *lights, uint32_t n)
+    {
+        require_scene();
+        if (n == 0) {
+            throw std::runtime_error("crtc_update_lights: no lights (the path tracer samples exactly one quad light per bounce)");
+        }
+        if (!lights) {
+            throw std::runtime_error("crtc_update_lights: lights is NULL");
+        }
+        staged_lights.assign(lights, lights + n);
+        lights_staged = true;
+    }
+    // Stream-ordered: frames enqueued before see the old scene, frames enqueued after the new one. Resets the
+    // accumulation as camera_changed does and drops the denoiser's history; nothing staged = nothing happens.
+    void commit_scene()
+    {
+        require_scene();
+        const bool geometry = scene_update && scene_update->staged();
+        if (!geometry && !lights_staged) {
+            return;
+        }
+        make_current();
+        if (geometry) {
+            scene_update->commit(d_nodes.ptr, d_tris.ptr, d_shade.ptr, stream, device);
+        }
+        if (lights_staged) {
+            const size_t n4 = staged_lights.size() * 5;
+            if (n4 > d_lights.count) {
+                CUDA_CHECK(cudaStreamSynchronize(stream));  // (frames in flight read the old buffer)
+                d_lights.alloc(n4);
+            }
+            CUDA_CHECK(cudaMemcpyAsync(d_lights.ptr, staged_lights.data(), staged_lights.size() * sizeof(crt_quad_light_t),
+                                       cudaMemcpyHostToDevice, stream));
+            num_lights = (uint32_t)staged_lights.size();
+            lights_staged = false;
+        }
+        CUDA_CHECK(cudaGetLastError());
+        frame_id = 0;  // as camera_changed: accum, AOVs and the adaptive block counts restart
+        adaptive_epoch = false;
+        if (!auto_decided) {
+            auto_frames = 0;  // an undecided any_far_first trial restarts
+        }
+        aov_state.drop_history();  // (its reprojection assumes static geometry)
     }
 
     // Enqueues one frame on the stream (no host synchronisation) and returns its record.
@@ -1448,6 +1525,11 @@ int crtc_set_option(crtc_renderer *r, const char *key, int64_t value)
             r->bvh_builder = (int)value;
         } else if (k == "count_traversal") {
             r->count_traversal = value != 0;
+        } else if (k == "dynamic_scene") {
+            if (value < 0 || value > 1) {
+                throw std::runtime_error("dynamic_scene must be 0 or 1");
+            }
+            r->dynamic_scene = value != 0;  // takes effect at the next crtc_set_scene
         } else if (k == "aov") {
             r->aov = value != 0;  // takes effect at the next crtc_initialize
         } else if (k == "denoise_history") {
@@ -1500,6 +1582,8 @@ int crtc_get_option(crtc_renderer *r, const char *key, int64_t *value)
             *value = r->build_rounds;  // PLOC rounds of the last device build
         } else if (k == "count_traversal") {
             *value = r->count_traversal ? 1 : 0;
+        } else if (k == "dynamic_scene") {
+            *value = r->dynamic_scene ? 1 : 0;
         } else if (k == "aov") {
             *value = r->aov ? 1 : 0;
         } else if (k == "denoise_history") {
@@ -1540,6 +1624,26 @@ int crtc_set_scene(crtc_renderer *r, const crt_scene_t *scene)
         }
         r->set_scene(scene);
     })
+}
+
+int crtc_update_instances(crtc_renderer *r, uint32_t first, uint32_t count, const float *transforms)
+{
+    CRTC_TRY({ require_renderer(r); r->require_dynamic("crtc_update_instances").stage_instances(first, count, transforms); })
+}
+
+int crtc_update_vertices(crtc_renderer *r, uint32_t mesh, uint32_t geometry, const float *vertices, uint32_t num_vertices)
+{
+    CRTC_TRY({ require_renderer(r); r->require_dynamic("crtc_update_vertices").stage_vertices(mesh, geometry, vertices, num_vertices); })
+}
+
+int crtc_update_lights(crtc_renderer *r, const crt_quad_light_t *lights, uint32_t num_lights)
+{
+    CRTC_TRY({ require_renderer(r); r->update_lights(lights, num_lights); })
+}
+
+int crtc_commit_scene(crtc_renderer *r)
+{
+    CRTC_TRY({ require_renderer(r); r->commit_scene(); })
 }
 
 int crtc_render(crtc_renderer *r, const float *pos, const float *dir, const float *up, float fovy, int camera_changed,

@@ -1,6 +1,7 @@
 // cuda_host_utils.h — small host-side helpers shared by the renderer object (crt_cuda_core.cu) and the device
 // set_scene driver (scene_device_build.cuh): error checking that throws like the reference does, an owning device
-// buffer, and a two-pass arena for groups of temporaries.
+// buffer, a two-pass arena for groups of temporaries, and a kernel launch that the host build of the renderer
+// (tests/simt_emu) compiles unchanged.
 #pragma once
 
 #include <algorithm>
@@ -89,5 +90,21 @@ struct ArenaBuf {
     explicit ArenaBuf(DeviceArena &a) : arena(&a) {}
     void alloc(size_t n) { ptr = static_cast<T *>(arena->take(std::max<size_t>(n, 1) * sizeof(T))); }
 };
+
+// A one-dimensional launch: chevrons under nvcc, simt::launch (simt_env.h, included first) in the host build of the
+// renderer, which compiles the headers that launch through this unchanged. An empty grid launches nothing.
+template <typename... P, typename... A>
+inline void launch(void (*kernel)(P...), unsigned grid, unsigned block, cudaStream_t stream, A... args)
+{
+    if (grid == 0) {
+        return;
+    }
+#ifdef __CUDACC__
+    kernel<<<grid, block, 0, stream>>>(args...);
+#else
+    (void)stream;
+    simt::launch(grid, block, [&] { kernel(args...); });
+#endif
+}
 
 }  // namespace crt_host

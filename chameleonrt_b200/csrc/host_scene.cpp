@@ -23,6 +23,8 @@ struct HostScene {
     size_t num_tris() const { return tri_shade.size(); }
 };
 
+}  // namespace
+
 // 4x4 inverse by cofactor expansion, column-major (the role of glm::inverse in
 // embree_utils.cpp:97).
 void mat4_inverse(const float *m, float *out)
@@ -66,6 +68,8 @@ void mat4_inverse(const float *m, float *out)
         out[i] = inv[i] * det;
     }
 }
+
+namespace {
 
 inline void normalize3(float *v)
 {

@@ -86,6 +86,8 @@ struct FlattenPlan {
     size_t total_tris = 0;
 };
 void plan_flatten(const crt_scene_t *scene, FlattenPlan &plan);
+// world_to_object from object_to_world (16 floats each, column-major), as plan_flatten computes it
+void mat4_inverse(const float *m, float *out);
 void pack_shading(const crt_scene_t *scene, int threads, ShadingRecords &out);
 
 }  // namespace crt

@@ -14,6 +14,7 @@
 #include "bvh8_traverse.h"
 #include "cuda_host_utils.h"
 #include "host_scene.h"
+#include "scene_update.cuh"
 
 namespace crt_host {
 
@@ -71,6 +72,8 @@ struct DeviceSceneBuild {
     DeviceBuffer<float4> *d_nodes = nullptr, *d_tris = nullptr, *d_shade = nullptr;
     std::vector<uint32_t> *leaf_flat_ids = nullptr;
     uint32_t num_nodes = 0, depth = 0;
+    std::vector<uint32_t> level_begin;     // as Bvh8::level_begin
+    SceneGeometry *geometry = nullptr;     // when set (option dynamic_scene): the uploaded geometry is kept there
     int rounds = 0;                        // PLOC rounds
     double build_ms = 0.0;                 // CUDA events around everything after the flattening
     double phase_ms[5] = {0, 0, 0, 0, 0};  // flatten (host wall clock), keys + sort, binary tree, BVH8 emission, packing
@@ -80,8 +83,9 @@ struct DeviceSceneBuild {
     {
         DeviceBuffer<float> d_verts;
         DeviceBuffer<float4> d_shade_in;
+        SceneGeometry local;
         const auto t0 = std::chrono::steady_clock::now();
-        flatten_on_device(scene, plan, d_verts, d_shade_in);  // (ends with a stream synchronisation)
+        flatten_on_device(scene, plan, geometry ? *geometry : local, d_verts, d_shade_in);  // (ends with a stream synchronisation)
         phase_ms[0] = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
         build_on_device((uint32_t)plan.total_tris, d_verts, d_shade_in);
     }
@@ -129,101 +133,23 @@ struct DeviceSceneBuild {
 
     // The triangle half of flatten_scene on the device: the unique geometries are uploaded once (not once per
     // instance) and k_flatten writes the world-space soup and the shading records in flattened order.
-    void flatten_on_device(const crt_scene_t *scene, const crt::FlattenPlan &plan, DeviceBuffer<float> &d_verts,
-                           DeviceBuffer<float4> &d_shade_in)
+    void flatten_on_device(const crt_scene_t *scene, const crt::FlattenPlan &plan, SceneGeometry &geom,
+                           DeviceBuffer<float> &d_verts, DeviceBuffer<float4> &d_shade_in)
     {
         const uint32_t total = (uint32_t)plan.total_tris;
-        struct Placed {
-            uint32_t vert_off, tri_off, uv_off;
-        };
-        std::vector<std::vector<Placed>> placed(scene->num_meshes);  // [mesh][geometry], filled on first use
-        std::vector<crt::DevSegment> segs;
-        size_t nv = 0, nt = 0, nuv = 0;
-        struct Copy {
-            const crt_geometry_t *geom;
-            Placed at;
-        };
-        std::vector<Copy> copies;
-        for (const crt::FlattenSegment &fs : plan.segments) {
-            const crt_mesh_t &mesh = scene->meshes[fs.mesh];
-            const crt_geometry_t &geom = mesh.geometries[fs.geometry];
-            if (geom.num_tris == 0) {
-                continue;
-            }
-            std::vector<Placed> &pm = placed[fs.mesh];
-            if (pm.empty()) {
-                pm.assign(mesh.num_geometries, Placed{crt::kB2Invalid, crt::kB2Invalid, crt::kB2Invalid});
-            }
-            Placed &pl = pm[fs.geometry];
-            if (pl.tri_off == crt::kB2Invalid) {
-                if (nv + geom.num_vertices >= 0xffffffffull || nt + geom.num_tris >= 0xffffffffull) {
-                    throw std::runtime_error("device set_scene: geometry arenas exceed 2^32 - 1 elements");
-                }
-                pl.vert_off = (uint32_t)nv;
-                pl.tri_off = (uint32_t)nt;
-                nv += geom.num_vertices;
-                nt += geom.num_tris;
-                if (geom.uvs) {
-                    pl.uv_off = (uint32_t)nuv;
-                    nuv += geom.num_vertices;
-                }
-                copies.push_back(Copy{&geom, pl});
-            }
-            crt::DevSegment ds;
-            ds.flat_base = (uint32_t)fs.flat_base;
-            ds.num_tris = geom.num_tris;
-            ds.vert_off = pl.vert_off;
-            ds.num_verts = geom.num_vertices;
-            ds.tri_off = pl.tri_off;
-            ds.uv_off = pl.uv_off;
-            ds.mat_id = fs.mat_id;
-            ds.instance = fs.instance;
-            segs.push_back(ds);
-        }
-        DeviceArena arena;
-        ArenaBuf<float> vert_arena(arena), uv_arena(arena), xforms(arena);
-        ArenaBuf<uint32_t> index_arena(arena), bad(arena);
-        ArenaBuf<crt::DevSegment> d_segs(arena);
-        auto carve = [&] {
-            vert_arena.alloc(nv * 3);
-            index_arena.alloc(nt * 3);
-            uv_arena.alloc(nuv * 2);
-            xforms.alloc((size_t)scene->num_instances * 32);
-            d_segs.alloc(segs.size());
-            bad.alloc(1);
-        };
-        carve();
-        arena.commit();
-        carve();
-        for (const Copy &c : copies) {
-            CUDA_CHECK(cudaMemcpyAsync(vert_arena.ptr + (size_t)c.at.vert_off * 3, c.geom->vertices,
-                                       (size_t)c.geom->num_vertices * 3 * sizeof(float), cudaMemcpyHostToDevice, stream));
-            CUDA_CHECK(cudaMemcpyAsync(index_arena.ptr + (size_t)c.at.tri_off * 3, c.geom->indices,
-                                       (size_t)c.geom->num_tris * 3 * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
-            if (c.geom->uvs) {
-                CUDA_CHECK(cudaMemcpyAsync(uv_arena.ptr + (size_t)c.at.uv_off * 2, c.geom->uvs,
-                                           (size_t)c.geom->num_vertices * 2 * sizeof(float), cudaMemcpyHostToDevice, stream));
-            }
-        }
-        std::vector<float> xf((size_t)scene->num_instances * 32);
-        for (uint32_t i = 0; i < scene->num_instances; ++i) {
-            std::memcpy(&xf[(size_t)i * 32], scene->instances[i].transform, 16 * sizeof(float));
-            std::memcpy(&xf[(size_t)i * 32 + 16], &plan.w2o_all[(size_t)i * 16], 16 * sizeof(float));
-        }
-        CUDA_CHECK(cudaMemcpyAsync(xforms.ptr, xf.data(), xf.size() * sizeof(float), cudaMemcpyHostToDevice, stream));
-        CUDA_CHECK(cudaMemcpyAsync(d_segs.ptr, segs.data(), segs.size() * sizeof(crt::DevSegment), cudaMemcpyHostToDevice, stream));
-        CUDA_CHECK(cudaMemsetAsync(bad.ptr, 0, sizeof(uint32_t), stream));
+        geom.upload(scene, plan, stream);
+        CUDA_CHECK(cudaMemsetAsync(geom.bad.ptr, 0, sizeof(uint32_t), stream));
         d_verts.alloc((size_t)total * 9);
         d_shade_in.alloc((size_t)total * 3);
         int sms = 0;
         CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
         const unsigned g = std::max(1u, std::min((total + crt::kBuildBlock - 1) / crt::kBuildBlock, (uint32_t)sms * 8u));
-        crt::k_flatten<<<g, crt::kBuildBlock, 0, stream>>>(d_segs.ptr, (uint32_t)segs.size(), xforms.ptr, vert_arena.ptr,
-                                                          index_arena.ptr, uv_arena.ptr, total, d_verts.ptr, d_shade_in.ptr,
-                                                          bad.ptr);
+        crt::k_flatten<<<g, crt::kBuildBlock, 0, stream>>>(geom.segs.ptr, geom.num_segs, geom.xforms.ptr, geom.vert_arena.ptr,
+                                                          geom.index_arena.ptr, geom.uv_arena.ptr, total, d_verts.ptr,
+                                                          d_shade_in.ptr, geom.bad.ptr);
         uint32_t bad_host = 0u;
-        CUDA_CHECK(cudaMemcpyAsync(&bad_host, bad.ptr, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
-        CUDA_CHECK(cudaStreamSynchronize(stream));  // also: the staging vectors and arenas go out of scope
+        CUDA_CHECK(cudaMemcpyAsync(&bad_host, geom.bad.ptr, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+        CUDA_CHECK(cudaStreamSynchronize(stream));
         if (bad_host) {
             throw std::runtime_error("triangle index out of range");
         }
@@ -381,8 +307,10 @@ struct DeviceSceneBuild {
         uint32_t *work = work0.ptr, *next_work = work1.ptr;
         uint32_t node_begin = 0, count = 1, tri_total = 0;
         depth = 0;
+        level_begin.clear();
         while (count) {
             ++depth;
+            level_begin.push_back(node_begin);
             if ((size_t)node_begin + count > max_nodes) {
                 throw DeviceBuildFailure("device BVH build: node count exceeds its bound");
             }
@@ -419,6 +347,7 @@ struct DeviceSceneBuild {
         }
         CUDA_CHECK(cudaEventRecord(ev_emitted, stream));
         num_nodes = node_begin;
+        level_begin.push_back(num_nodes);
         d_nodes->alloc((size_t)num_nodes * 5);
         CUDA_CHECK(cudaMemcpyAsync(d_nodes->ptr, nodes_tmp.ptr, (size_t)num_nodes * 80, cudaMemcpyDeviceToDevice, stream));
         d_tris->alloc((size_t)n * 3);

@@ -116,6 +116,11 @@ void crtc_destroy(crtc_renderer *r);
  *                 range is an error. Nothing runs in the frame path: two more kernels run inside crtc_denoise only. Memory:
  *                 the first crtc_denoise adds 80 B per framebuffer pixel (two history buffers of 10 floats; 1920x1080:
  *                 166 MB). crtc_initialize and crtc_set_scene drop the history.
+ *   "dynamic_scene" 0 (default) / 1: crtc_set_scene keeps on the device what crtc_update_instances / crtc_update_vertices
+ *                 and crtc_commit_scene need. Takes effect at the next crtc_set_scene; with 0 nothing is kept and nothing
+ *                 more runs. Every builder ("bvh_builder" 0, 1, 2). Memory: the unique geometry (12 B per unique vertex,
+ *                 + 8 B if it has uvs; 12 B per unique triangle; 128 B per instance; 32 B per (instance, geometry) pair),
+ *                 36 B per flattened triangle and 32 B per BVH8 node.
  */
 int crtc_set_option(crtc_renderer *r, const char *key, int64_t value);
 
@@ -136,6 +141,45 @@ int crtc_initialize(crtc_renderer *r, int fb_width, int fb_height);
 /* RenderBackend::set_scene: flattens instances, builds the BVH8 on the host, uploads
  * geometry / materials / textures / lights, resets accumulation. */
 int crtc_set_scene(crtc_renderer *r, const crt_scene_t *scene);
+
+/* Scene updates between frames, without a new crtc_set_scene: instances move, meshes deform, lights change. The update
+ * calls only stage; crtc_commit_scene applies everything staged at once. The caller's arrays may be reused as soon as an
+ * update call returns. crtc_set_scene discards staged updates.
+ *   Topology is fixed: indices, uvs, materials, textures and the instance -> mesh mapping stay those of crtc_set_scene.
+ *   Result: after a commit, frames, crtc_trace_closest and crtc_trace_any are bit-identical to those of a renderer that
+ *   was crtc_set_scene'd with the updated scene (same options). The BVH8 keeps its topology and leaf order and its boxes
+ *   are refit on the device (DESIGN.md section 2, "Scene updates"); a tree refit after large motions traces slower than
+ *   a new build of the moved scene (profiles/dynamic_h100.md): crtc_set_scene is the way to get a new tree.
+ * Every call fails if no scene has been set.
+ *
+ * crtc_update_instances: needs option dynamic_scene = 1 at the last crtc_set_scene. Instances first .. first + count - 1
+ * get new object_to_world matrices, 16 floats each, column-major as crt_instance_t::transform. world_to_object is
+ * computed on the host as crtc_set_scene computes it, so any matrix crtc_set_scene accepts (singular or non-finite
+ * included) gives the same result as there. Fails if first + count exceeds the instance count or transforms is NULL
+ * with count > 0. */
+int crtc_update_instances(crtc_renderer *r, uint32_t first, uint32_t count, const float *transforms);
+/* crtc_update_vertices: needs option dynamic_scene = 1 at the last crtc_set_scene. New positions of the vertices of
+ * geometry `geometry` of mesh `mesh` (3 floats each, object space); every instance of the mesh moves with them. Fails if
+ * the mesh or geometry id is out of range, if num_vertices differs from the geometry's vertex count at crtc_set_scene, or
+ * if vertices is NULL with num_vertices > 0. A geometry that no instance references with triangles is accepted and the
+ * update does nothing. Staging the same geometry twice keeps the later positions. */
+int crtc_update_vertices(crtc_renderer *r, uint32_t mesh, uint32_t geometry, const float *vertices, uint32_t num_vertices);
+/* crtc_update_lights: no option needed. Replaces all lights (crt_quad_light_t records, as crt_scene_t::lights); the
+ * count may change. Fails if num_lights is 0 (as crtc_set_scene does) or lights is NULL. */
+int crtc_update_lights(crtc_renderer *r, const crt_quad_light_t *lights, uint32_t num_lights);
+/* crtc_commit_scene: applies the staged updates. Enqueued on the renderer's stream (crtc_set_stream applies) without
+ * waiting for frames in flight: frames enqueued before see the old scene, frames enqueued after the new one (the
+ * staged data is copied from pageable memory; a light count above every earlier one waits for the stream once). Every
+ * commit with staged instances or vertices re-flattens every triangle (k_reflatten) and refits every node (one
+ * k_bvh8_refit launch per BVH8 level). Then:
+ *   - the accumulation resets as on camera_changed: accum, the AOVs and the adaptive block counts; the next frame equals
+ *     frame 0 of a fresh renderer;
+ *   - the denoiser's history is dropped (its reprojection assumes static geometry): crtc_read_denoise_history fails until
+ *     the next crtc_denoise;
+ *   - the any_far_first decision is kept; if mode 2 has not decided yet, its trial restarts as after crtc_set_scene;
+ *   - frame counters and stage times do not include the commit's launches.
+ * With nothing staged it does nothing: no reset, no launch. */
+int crtc_commit_scene(crtc_renderer *r);
 
 /* RenderBackend::render. pos/dir/up: 3 floats each; fovy in degrees. If
  * readback_framebuffer != 0 and img != NULL, img receives fb_width*fb_height RGBA8 pixels
