@@ -126,7 +126,7 @@ class RenderCUDA:
                  count_traversal: bool = False, bvh_threads: int = 0, stream: Optional[int] = None,
                  any_far_first: Optional[int] = None, bvh_builder: Optional[str] = None,
                  tri_pass_defer: Optional[int] = None, shade_sort: Optional[int] = None, aov: bool = False,
-                 denoise_history: int = 0, dynamic_scene: bool = False):
+                 denoise_history: int = 0, dynamic_scene: bool = False, denoise_motion: bool = False):
         self.lib = load_lib()
         self.h = C.c_void_p()
         self._check(self.lib.crtc_create(C.byref(self.h), device))
@@ -168,6 +168,8 @@ class RenderCUDA:
             self._check(self.lib.crtc_set_option(self.h, b"denoise_history", int(denoise_history)))
         if dynamic_scene:  # set_scene keeps what update_instances / update_vertices + commit_scene need (option "dynamic_scene")
             self._check(self.lib.crtc_set_option(self.h, b"dynamic_scene", 1))
+        if denoise_motion:  # commit_scene keeps denoise()'s history, moved with the geometry (option "denoise_motion")
+            self._check(self.lib.crtc_set_option(self.h, b"denoise_motion", 1))
         if stream is not None:
             self._check(self.lib.crtc_set_stream(self.h, C.c_void_p(stream)))
         self.width = self.height = 0

@@ -2,8 +2,13 @@
 //
 //   k_aov_primary   after the primary-ray traversal, before k_shade(0): albedo, coverage, normal and depth of the primary
 //                   hits, folded into a per-pixel running mean with k_resolve's formula
+//   k_aov_hit       (option denoise_motion, dynamic scenes) in an epoch's first wavefront, after the primary traversal:
+//                   each pixel's first hit triangle and barycentrics, for k_dn_temporal<true>
 //   k_aov_moments   after k_resolve: the first two moments of the per-sample luminance, same running mean
 //   k_dn_prepare    demodulated radiance, variance of the pixel mean, unit normals, depth and its screen gradient
+//   k_dn_temporal   (option denoise_history) the temporal half of SVGF: reprojects the history into this epoch; with
+//                   <true>, through the motion of each pixel's triangle since the history was written
+//   k_dn_variance   (option denoise_history) the variance from the integrated moments
 //   k_dn_atrous     one à-trous iteration of the spatial part of SVGF (Schied et al. 2017); the last one remodulates and
 //                   writes float RGB and sRGB8
 //
@@ -19,6 +24,7 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 
+#include "bvh8_device.cuh"
 #include "cuda_host_utils.h"
 #include "kernels.cuh"
 
@@ -100,6 +106,32 @@ __global__ void __launch_bounds__(128, 4) k_aov_primary(DeviceScene sc, FrameLay
             aov_full[(size_t)kAovFloats * p + j] = acc[j];
         }
     }
+}
+
+// Option "denoise_motion", on a dynamic scene, in the first wavefront of an epoch only (frame 0 is its first frame):
+// one thread per local pixel writes the pixel's hit record, 3 words at the full-frame position: bits(leaf-order
+// triangle), u, v of the first sample of frame 0, in sample order, that hit geometry; bits(kMiss), 0, 0 if none did.
+__global__ void __launch_bounds__(256) k_aov_hit(FrameLayout f, PathState ps, float *hit_full)
+{
+    const uint32_t lp = blockIdx.x * blockDim.x + threadIdx.x;
+    uint32_t x, y;
+    if (lp >= f.npx_local || !local_pixel_coords(f, lp, x, y)) {
+        return;
+    }
+    float rec[3] = {__uint_as_float(kMiss), 0.f, 0.f};
+    for (uint32_t s = 0; s < f.spp; ++s) {
+        const float4 h = ps.hit[(size_t)s * f.npx_local + lp];
+        if (__float_as_uint(h.w) != kMiss) {
+            rec[0] = h.w;
+            rec[1] = h.y;
+            rec[2] = h.z;
+            break;
+        }
+    }
+    float *o = hit_full + 3 * ((size_t)y * f.fb_w + x);
+    o[0] = rec[0];
+    o[1] = rec[1];
+    o[2] = rec[2];
 }
 
 // Mean of L and L^2 over each frame's spp samples (L: luminance of the sample's radiance), folded like k_resolve.
@@ -253,12 +285,42 @@ struct HistoryView {
     float minv[9];
 };
 
+// Option "denoise_motion": the live geometry of a dynamic scene (scene_update.cuh, SceneGeometry), as the denoiser
+// reads it. num_xforms / num_verts count floats.
+struct LiveGeometry {
+    const DevSegment *segs;
+    uint32_t num_segs;
+    const uint32_t *leaf_flat_ids, *index_arena;
+    const float *uv_arena, *xforms, *verts;
+    size_t num_xforms, num_verts;
+};
+
+// What k_dn_temporal<true> needs to move a pixel's point with its triangle: the live geometry (its segments, index and
+// uv arenas and leaf order also serve the snapshot: a commit does not change them) and the snapshot taken with `prev`.
+struct DenoiseMotion {
+    const float *hit;  // k_aov_hit's records of this epoch
+    LiveGeometry live;
+    const float *prev_xforms, *prev_verts;
+};
+
+// The world point at barycentrics (b1, b2) of a triangle's world vertices w (9 floats)
+CRT_D float3 dn_bary_point(const float *w, float b1, float b2)
+{
+    return mk3(w[0] + b1 * (w[3] - w[0]) + b2 * (w[6] - w[0]), w[1] + b1 * (w[4] - w[1]) + b2 * (w[7] - w[1]),
+               w[2] + b1 * (w[5] - w[2]) + b2 * (w[8] - w[2]));
+}
+
 // One thread per pixel, after k_dn_prepare. Reprojects the pixel's first hit into the previous camera, blends the
 // valid bilinear taps of `prev` (null: no history) with this epoch's accum and moments, writes the result to `cur` and
 // the blended colour to iv.xyz. Pixels without history keep k_dn_prepare's iv bits.
+// MOTION (the geometry changed since `prev` was written): a pixel with a hit record whose triangle moved has its point
+// moved by the triangle's displacement at the record's barycentrics, and its taps' normals compared with the previous
+// triangle's normal on nhat_p's side; every other pixel takes the static arithmetic. <false> ignores `mo`.
+template <bool MOTION>
 __global__ void __launch_bounds__(kDenoiseBlock) k_dn_temporal(int w, int h, float samples, float max_history, ViewParams view,
                                                                HistoryView pv, const float *prev, const float *aov,
-                                                               const float4 *guide, float4 *iv, float *cur)
+                                                               const float4 *guide, float4 *iv, float *cur,
+                                                               DenoiseMotion mo)
 {
     const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= (uint32_t)w * (uint32_t)h) {
@@ -277,13 +339,44 @@ __global__ void __launch_bounds__(kDenoiseBlock) k_dn_temporal(int w, int h, flo
         const float3 d = normalize(mk3(view.dir_du.x * px_x + view.dir_dv.x * px_y + view.dir_top_left.x,
                                        view.dir_du.y * px_x + view.dir_dv.y * px_y + view.dir_top_left.y,
                                        view.dir_du.z * px_x + view.dir_dv.z * px_y + view.dir_top_left.z));
-        const float3 r = mk3(view.pos.x + gp.w * d.x, view.pos.y + gp.w * d.y, view.pos.z + gp.w * d.z) - pv.pos;
+        float3 X = mk3(view.pos.x + gp.w * d.x, view.pos.y + gp.w * d.y, view.pos.z + gp.w * d.z);
+        float3 n_ref = np;  // what the taps' normals are compared with
+        bool moved_ok = true;
+        if (MOTION) {
+            const float *rec = mo.hit + 3 * (size_t)p;
+            const uint32_t tri = __float_as_uint(rec[0]);
+            if (tri != kMiss) {
+                const LiveGeometry &g = mo.live;
+                const uint32_t f = g.leaf_flat_ids[tri];
+                const DevSegment seg = g.segs[dev_find_segment(g.segs, g.num_segs, f)];
+                float wc[9], wp[9];
+                float4 sc[3], sp[3];
+                dev_flatten_triangle(seg, f, g.xforms, g.verts, g.index_arena, g.uv_arena, wc, sc);
+                dev_flatten_triangle(seg, f, mo.prev_xforms, mo.prev_verts, g.index_arena, g.uv_arena, wp, sp);
+                bool same = true;
+#pragma unroll
+                for (int k = 0; k < 9; ++k) {
+                    same = same && __float_as_uint(wc[k]) == __float_as_uint(wp[k]);
+                }
+                if (!same) {
+                    const float3 P = dn_bary_point(wc, rec[1], rec[2]), Pp = dn_bary_point(wp, rec[1], rec[2]);
+                    const float3 dp = Pp - P;
+                    const float inf = __uint_as_float(0x7f800000u);
+                    moved_ok = fabsf(dp.x) < inf && fabsf(dp.y) < inf && fabsf(dp.z) < inf;
+                    X = X + dp;
+                    const float s = dot(np, mk3(sc[0].x, sc[0].y, sc[0].z)) < 0.f ? -1.f : 1.f;
+                    n_ref = mk3(s * sp[0].x, s * sp[0].y, s * sp[0].z);
+                }
+            }
+        }
+        const float3 r = X - pv.pos;
         const float al = pv.minv[0] * r.x + pv.minv[1] * r.y + pv.minv[2] * r.z;
         const float be = pv.minv[3] * r.x + pv.minv[4] * r.y + pv.minv[5] * r.z;
         const float ga = pv.minv[6] * r.x + pv.minv[7] * r.y + pv.minv[8] * r.z;
         const float sx = (al / ga) * (float)w - 0.5f, sy = (be / ga) * (float)h - 0.5f;
-        // (outside this window every tap is outside the image; it also keeps NaN and huge values away from the int cast)
-        if (ga > 0.f && sx > -1.f && sx < (float)w && sy > -1.f && sy < (float)h) {
+        // (outside this window every tap is outside the image; it also keeps NaN and huge values away from the int cast;
+        // a non-finite displacement leaves the pixel without history)
+        if (moved_ok && ga > 0.f && sx > -1.f && sx < (float)w && sy > -1.f && sy < (float)h) {
             const float dist = length(r);
             const float fx0 = floorf(sx), fy0 = floorf(sy);
             const float fx = sx - fx0, fy = sy - fy0;
@@ -309,7 +402,7 @@ __global__ void __launch_bounds__(kDenoiseBlock) k_dn_temporal(int w, int h, flo
                 const float zy = prev[(size_t)kHistFloats * ((size_t)yd * w + qx) + kHistDepth] -
                                  prev[(size_t)kHistFloats * ((size_t)yu * w + qx) + kHistDepth];
                 const float gx = xr - xl == 2 ? 0.5f * zx : zx, gy = yd - yu == 2 ? 0.5f * zy : zy;
-                if (!(fabsf(hq[kHistDepth] - dist) <= 0.02f * dist + 2.f * (fabsf(gx) + fabsf(gy))) || !(dot(np, nq) >= 0.9f)) {
+                if (!(fabsf(hq[kHistDepth] - dist) <= 0.02f * dist + 2.f * (fabsf(gx) + fabsf(gy))) || !(dot(n_ref, nq) >= 0.9f)) {
                     continue;
                 }
                 const float wt = ((t & 1) ? fx : 1.f - fx) * ((t >> 1) ? fy : 1.f - fy);
@@ -405,16 +498,33 @@ struct DenoiseParams {
     float sigma_l = 4.f, sigma_n = 128.f, sigma_z = 1.f;
 };
 
-// What a history buffer was written for: the reset epoch and the camera of that epoch's first frame
+// What a history buffer was written for: the reset epoch, the camera of that epoch's first frame and the renderer's
+// geometry version (bumped by crtc_set_scene and by every commit that moves geometry)
 struct HistoryTag {
     bool valid = false;
     uint64_t epoch = 0;
     ViewParams view{};
+    uint64_t geometry = 0;
+};
+
+// A copy of the moving part of the geometry (instance matrices, unique vertices), taken when its history buffer was
+// written under geometry version `version`
+struct GeometrySnapshot {
+    crt_host::DeviceBuffer<float> xforms, verts;
+    bool valid = false;
+    uint64_t version = 0;
+    void release()
+    {
+        xforms.release();
+        verts.release();
+        valid = false;
+    }
 };
 
 // The renderer's AOV and denoiser state. AOV buffers: 40 B per local pixel (tile-padded) + 40 B per framebuffer pixel;
 // denoiser buffers, allocated by the first denoise call: 72 B per framebuffer pixel, + 80 B with option denoise_history
-// (the two history buffers, `prev` and `cur`).
+// (the two history buffers, `prev` and `cur`). Option denoise_motion, dynamic scenes only: 12 B per framebuffer pixel
+// (hit records) + per history buffer a geometry snapshot of 128 B per instance and 12 B per unique vertex.
 struct AovState {
     crt_host::DeviceBuffer<float> local, full;
     crt_host::DeviceBuffer<float4> dn_iv[2], dn_guide;
@@ -424,6 +534,8 @@ struct AovState {
     crt_host::DeviceBuffer<float> hist[2];  // hist[hist_cur] is `cur`, the other one `prev`
     HistoryTag hist_tag[2];
     int hist_cur = 0;
+    crt_host::DeviceBuffer<float> hit;  // k_aov_hit's records, 3 words per framebuffer pixel
+    GeometrySnapshot snap[2];           // snap[i] goes with hist[i]
 
     void drop_history()
     {
@@ -442,6 +554,9 @@ struct AovState {
         dn_img.release();
         hist[0].release();
         hist[1].release();
+        hit.release();
+        snap[0].release();
+        snap[1].release();
         drop_history();
     }
     // `cur` if the last denoise call was made in `epoch`, else null
@@ -497,6 +612,12 @@ struct AovState {
             crt_host::launch(k_aov_primary<false>, g, 128, stream, sc, f, ps, frame_id, local.ptr, full.ptr);
         }
     }
+    // Option denoise_motion: the hit records of an epoch's first wavefront (allocated on first use)
+    void launch_hit(const FrameLayout &f, const PathState &ps, cudaStream_t stream)
+    {
+        hit.alloc((size_t)3 * f.fb_w * f.fb_h);
+        crt_host::launch(k_aov_hit, (f.npx_local + 255) / 256, 256, stream, f, ps, hit.ptr);
+    }
     void launch_moments(const FrameLayout &f, const PathState &ps, uint32_t frame_id, cudaStream_t stream)
     {
         crt_host::launch(k_aov_moments, (f.npx_local + 255) / 256, 256, stream, f, ps, frame_id, local.ptr, full.ptr);
@@ -504,9 +625,11 @@ struct AovState {
     // Denoises the full frame `accum` (w x h x 3, `samples` = spp * frames accumulated) into dn_rgb / dn_img.
     // max_history > 0 (option denoise_history): the temporal pass runs between k_dn_prepare and the a-trous chain, with
     // the history of the latest earlier epoch that had a denoise call as `prev`; `epoch` and `view` are the current
-    // reset epoch and the camera of its first frame.
+    // reset epoch and the camera of its first frame. `geometry` is the renderer's geometry version; `live` (option
+    // denoise_motion on a dynamic scene, else null) lets a history written under another version reproject through the
+    // motion of each pixel's triangle, and has `cur` keep a snapshot of the geometry it was written under.
     void denoise(int w, int h, float samples, const float *accum, const DenoiseParams &prm, uint32_t max_history,
-                 uint64_t epoch, const ViewParams &view, cudaStream_t stream)
+                 uint64_t epoch, const ViewParams &view, uint64_t geometry, const LiveGeometry *live, cudaStream_t stream)
     {
         const size_t n = (size_t)w * h;
         if (dn_img.count != n || (max_history && hist[0].count != kHistFloats * n)) {
@@ -531,16 +654,46 @@ struct AovState {
                 hist_cur ^= 1;  // cur -> prev; the older prev is overwritten
             }
             const HistoryTag &pt = hist_tag[hist_cur ^ 1];
+            const GeometrySnapshot &ps = snap[hist_cur ^ 1];
             HistoryView pv{};
-            const bool have_prev = pt.valid && pt.epoch < epoch && history_view(pt.view, pv);
-            crt_host::launch(k_dn_temporal, g, kDenoiseBlock, stream, w, h, samples, (float)max_history, view, pv,
-                       have_prev ? (const float *)hist[hist_cur ^ 1].ptr : nullptr, (const float *)full.ptr,
-                       (const float4 *)dn_guide.ptr, dn_iv[0].ptr, hist[hist_cur].ptr);
+            bool have_prev = pt.valid && pt.epoch < epoch && history_view(pt.view, pv);
+            const bool moved = have_prev && pt.geometry != geometry;
+            DenoiseMotion mo{};
+            if (moved) {
+                // (a history of other geometry reprojects only through its snapshot; without one it is not carried)
+                have_prev = live && ps.valid && ps.version == pt.geometry && hit.count == (size_t)3 * n;
+                if (have_prev) {
+                    mo = DenoiseMotion{hit.ptr, *live, ps.xforms.ptr, ps.verts.ptr};
+                }
+            }
+            const float *prev = have_prev ? (const float *)hist[hist_cur ^ 1].ptr : nullptr;
+            if (moved && have_prev) {
+                crt_host::launch(k_dn_temporal<true>, g, kDenoiseBlock, stream, w, h, samples, (float)max_history, view, pv,
+                                 prev, (const float *)full.ptr, (const float4 *)dn_guide.ptr, dn_iv[0].ptr,
+                                 hist[hist_cur].ptr, mo);
+            } else {
+                crt_host::launch(k_dn_temporal<false>, g, kDenoiseBlock, stream, w, h, samples, (float)max_history, view, pv,
+                                 prev, (const float *)full.ptr, (const float4 *)dn_guide.ptr, dn_iv[0].ptr,
+                                 hist[hist_cur].ptr, mo);
+            }
             crt_host::launch(k_dn_variance, g, kDenoiseBlock, stream, w, h, prm.sigma_n, prm.sigma_z, (const float *)hist[hist_cur].ptr,
                        (const float4 *)dn_guide.ptr, (const float2 *)dn_grad.ptr, dn_iv[0].ptr);
             hist_tag[hist_cur].valid = true;
             hist_tag[hist_cur].epoch = epoch;
             hist_tag[hist_cur].view = view;
+            hist_tag[hist_cur].geometry = geometry;
+            GeometrySnapshot &cs = snap[hist_cur];
+            if (live && !(cs.valid && cs.version == geometry)) {
+                // (stream-ordered after k_dn_temporal, which read the other snapshot)
+                cs.xforms.alloc(live->num_xforms);
+                cs.verts.alloc(live->num_verts);
+                CUDA_CHECK(cudaMemcpyAsync(cs.xforms.ptr, live->xforms, live->num_xforms * sizeof(float),
+                                           cudaMemcpyDeviceToDevice, stream));
+                CUDA_CHECK(cudaMemcpyAsync(cs.verts.ptr, live->verts, live->num_verts * sizeof(float),
+                                           cudaMemcpyDeviceToDevice, stream));
+                cs.valid = true;
+                cs.version = geometry;
+            }
         }
         for (int i = 0; i < prm.iterations; ++i) {
             const float4 *in = dn_iv[i & 1].ptr;

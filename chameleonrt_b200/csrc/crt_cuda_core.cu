@@ -244,6 +244,17 @@ struct crtc_renderer {
     uint32_t dn_history = 0, dn_history_active = 0;
     uint64_t epoch = 0;
     crt::ViewParams epoch_view{};
+    // option "denoise_motion": a commit that moves geometry keeps the history, reprojected through each pixel's triangle;
+    // `dn_motion_active` is what the last crtc_initialize set up. `geometry_version` counts crtc_set_scene calls and
+    // commits with staged instances or vertices.
+    bool dn_motion = false, dn_motion_active = false;
+    uint64_t geometry_version = 0;
+    // The frame index the current epoch's samples start from (k_raygen's seeds): 0 after every reset, except that a
+    // commit keeping the history (option denoise_motion) continues from where the epoch before it ended, so that a still
+    // pixel draws new samples instead of re-rendering the ones its history already holds. A camera_changed render
+    // right after such a commit does not restart it.
+    uint32_t sample_base = 0;
+    bool motion_frames() const { return dn_motion_active && scene_update != nullptr; }
     void require_unshared_aov(const char *what) const
     {
         if (aov_active) {
@@ -666,6 +677,9 @@ struct crtc_renderer {
             throw std::runtime_error("initialize: option denoise_history needs option aov = 1 (the history is built from the "
                                      "first-hit AOVs)");
         }
+        if (dn_motion && !dn_history) {
+            throw std::runtime_error("initialize: option denoise_motion needs option denoise_history > 0");
+        }
         if (aov && adaptive) {
             throw std::runtime_error("initialize: option aov cannot be combined with adaptive sampling (the AOVs and the "
                                      "denoiser assume the same number of samples in every pixel); turn it off with "
@@ -677,6 +691,7 @@ struct crtc_renderer {
         close_peer_frame();      // the frame's shape (and on the exporting rank, its buffers) change:
         frame_exported = false;  // crtc_export_frame / crtc_import_frame must be called again
         frame_id = 0;
+        sample_base = 0;
         fb_w = w;
         fb_h = h;
         ntx = crt::tiles_along(w);
@@ -696,6 +711,7 @@ struct crtc_renderer {
         CUDA_CHECK(cudaMemsetAsync(d_img_full.ptr, 0, ((size_t)w * h + crt::kSyncWords) * 4, stream));
         aov_active = aov;
         dn_history_active = dn_history;
+        dn_motion_active = dn_motion;
         if (aov_active) {  // (drops the denoiser's history too)
             aov_state.allocate(npx_local, (size_t)w * h, stream);
         } else {
@@ -716,6 +732,7 @@ struct crtc_renderer {
         lights_staged = false;
         staged_lights.clear();
         frame_id = 0;
+        sample_base = 0;
         adaptive_epoch = false;
         auto_frames = 0;
         auto_decided = false;
@@ -818,6 +835,7 @@ struct crtc_renderer {
             }
         }
         aov_state.drop_history();  // (a history of another scene does not reproject)
+        ++geometry_version;
         scene_update = std::move(keep);
     }
 
@@ -843,12 +861,13 @@ struct crtc_renderer {
         lights_staged = true;
     }
     // Stream-ordered: frames enqueued before see the old scene, frames enqueued after the new one. Resets the
-    // accumulation as camera_changed does and drops the denoiser's history; nothing staged = nothing happens.
+    // accumulation as camera_changed does and drops the denoiser's history (kept with option denoise_motion unless
+    // lights change); nothing staged = nothing happens.
     void commit_scene()
     {
         require_scene();
-        const bool geometry = scene_update && scene_update->staged();
-        if (!geometry && !lights_staged) {
+        const bool geometry = scene_update && scene_update->staged(), lights = lights_staged;
+        if (!geometry && !lights) {
             return;
         }
         make_current();
@@ -867,12 +886,20 @@ struct crtc_renderer {
             lights_staged = false;
         }
         CUDA_CHECK(cudaGetLastError());
+        if (geometry) {
+            ++geometry_version;
+        }
+        if (lights || !motion_frames()) {
+            aov_state.drop_history();  // (new lights change the radiance everywhere; without motion, nothing reprojects)
+            sample_base = 0;
+        } else {
+            sample_base += frame_id;
+        }
         frame_id = 0;  // as camera_changed: accum, AOVs and the adaptive block counts restart
         adaptive_epoch = false;
         if (!auto_decided) {
             auto_frames = 0;  // an undecided any_far_first trial restarts
         }
-        aov_state.drop_history();  // (its reprojection assumes static geometry)
     }
 
     // Enqueues one frame on the stream (no host synchronisation) and returns its record.
@@ -892,10 +919,13 @@ struct crtc_renderer {
         }
         make_current();
         if (camera_changed) {
+            if (frame_id != 0) {  // (right after a commit, the commit's epoch goes on)
+                sample_base = 0;
+            }
             frame_id = 0;  // render_embree.cpp:145-147
             adaptive_epoch = false;
         }
-        const crt::ViewParams view = crt::make_view_params(pos, dir, up, fovy, fb_w, fb_h, frame_id);
+        const crt::ViewParams view = crt::make_view_params(pos, dir, up, fovy, fb_w, fb_h, sample_base + frame_id);
         if (frame_id == 0) {  // the first frame since a reset starts a new epoch (crtc_denoise's history)
             ++epoch;
             epoch_view = view;
@@ -978,6 +1008,10 @@ struct crtc_renderer {
             if (aov_active) {  // (its time counts as shading: the next mark closes the stage)
                 aov_state.launch_primary(sc, fl, ps, frame_id, stream);
                 rec.launches += 1;
+                if (frame_id == 0 && motion_frames()) {  // (the same)
+                    aov_state.launch_hit(fl, ps, stream);
+                    rec.launches += 1;
+                }
             }
             for (int b = 0; b < max_depth; ++b) {
                 const uint32_t *qin = ps.queue[b & 1];
@@ -1351,8 +1385,14 @@ struct crtc_renderer {
         }
         require_aov_frame("crtc_denoise");
         make_current();
+        crt::LiveGeometry live{};
+        if (motion_frames()) {
+            const crt_host::SceneGeometry &g = *scene_update->geometry;
+            live = crt::LiveGeometry{g.segs.ptr, g.num_segs, scene_update->leaf_flat_ids.ptr, g.index_arena.ptr, g.uv_arena.ptr,
+                                     g.xforms.ptr, g.vert_arena.ptr, g.xf.size(), g.vert_floats};
+        }
         aov_state.denoise(fb_w, fb_h, (float)spp * (float)frame_id, d_accum_full.ptr, p, dn_history_active, epoch, epoch_view,
-                          stream);
+                          geometry_version, motion_frames() ? &live : nullptr, stream);
         const size_t n = (size_t)fb_w * fb_h;
         if (rgb_out) {
             CUDA_CHECK(cudaMemcpyAsync(rgb_out, aov_state.dn_rgb.ptr, n * 3 * sizeof(float), cudaMemcpyDeviceToHost, stream));
@@ -1537,6 +1577,11 @@ int crtc_set_option(crtc_renderer *r, const char *key, int64_t value)
                 throw std::runtime_error("denoise_history must be in [0, 1024] (0 = off)");
             }
             r->dn_history = (uint32_t)value;  // takes effect at the next crtc_initialize
+        } else if (k == "denoise_motion") {
+            if (value < 0 || value > 1) {
+                throw std::runtime_error("denoise_motion must be 0 or 1");
+            }
+            r->dn_motion = value != 0;  // takes effect at the next crtc_initialize
         } else if (k == "refill_idle") {
             r->refill_idle = (int)std::min<int64_t>(std::max<int64_t>(value, 1), 32);
         } else if (k == "any_far_first") {
@@ -1588,6 +1633,8 @@ int crtc_get_option(crtc_renderer *r, const char *key, int64_t *value)
             *value = r->aov ? 1 : 0;
         } else if (k == "denoise_history") {
             *value = r->dn_history;
+        } else if (k == "denoise_motion") {
+            *value = r->dn_motion ? 1 : 0;
         } else if (k == "refill_idle") {
             *value = r->refill_idle;
         } else if (k == "any_far_first") {

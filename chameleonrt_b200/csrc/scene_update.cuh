@@ -147,6 +147,7 @@ struct SceneGeometry {
     ArenaBuf<uint32_t> index_arena{arena}, bad{arena};
     ArenaBuf<crt::DevSegment> segs{arena};
     uint32_t num_segs = 0;
+    size_t vert_floats = 0;                   // floats in vert_arena
     std::vector<std::vector<Placed>> placed;  // [mesh][geometry]; empty: no geometry of the mesh is in the arenas
     std::vector<float> xf;                    // 32 floats per instance, as `xforms`
 
@@ -202,6 +203,7 @@ struct SceneGeometry {
             host_segs.push_back(ds);
         }
         num_segs = (uint32_t)host_segs.size();
+        vert_floats = nv * 3;
         auto carve = [&] {
             vert_arena.alloc(nv * 3);
             index_arena.alloc(nt * 3);

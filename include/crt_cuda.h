@@ -108,6 +108,8 @@ void crtc_destroy(crtc_renderer *r);
  *                 k_aov_moments after the resolve), so counter [2] (kernel launches) grows by 2 per wavefront; their
  *                 times are counted in stage [2] (shade) and [5] (resolve) of crtc_get_stage_times. They read the path
  *                 state and write only their own buffers: accum, img and the ray counts are the same with the option on.
+ *                 With option denoise_motion on a dynamic scene, an epoch's first wavefront (the first after a reset) runs
+ *                 a third one, k_aov_hit (counted in stage [2]), so counter [2] grows by 3 there.
  *                 Memory: 40 B per pixel of the local tiles (64x64-padded) + 40 B per framebuffer pixel; the first
  *                 crtc_denoise adds 72 B per framebuffer pixel (1920x1080: 166 MB of AOVs + 149 MB for the denoiser).
  *   "denoise_history" H in 0..1024, 0 (default) = off: crtc_denoise carries a temporal history across accumulation
@@ -116,6 +118,21 @@ void crtc_destroy(crtc_renderer *r);
  *                 range is an error. Nothing runs in the frame path: two more kernels run inside crtc_denoise only. Memory:
  *                 the first crtc_denoise adds 80 B per framebuffer pixel (two history buffers of 10 floats; 1920x1080:
  *                 166 MB). crtc_initialize and crtc_set_scene drop the history.
+ *   "denoise_motion" 0 (default) / 1: a crtc_commit_scene that moves geometry keeps the denoiser's history; the next
+ *                 crtc_denoise reprojects each pixel through the motion of the triangle it sees (crtc_denoise, step b').
+ *                 Takes effect at the next crtc_initialize, which fails if it is 1 with option denoise_history = 0; any
+ *                 other value than 0 or 1 is an error. Acts only on scenes set with dynamic_scene = 1: with a static scene
+ *                 nothing is allocated and nothing runs. On a dynamic scene: one more kernel in an epoch's first
+ *                 wavefront (see "aov"); memory: 12 B per framebuffer pixel (each pixel's hit record) and, from the first
+ *                 crtc_denoise, two geometry snapshots of 128 B per instance + 12 B per unique vertex, one per history
+ *                 buffer (C3: 961 instances, ~2 x 0.1 MB + the vertices). Commits that change lights still drop the
+ *                 history. After a commit that keeps the history, the sample sequence is not restarted: the frames
+ *                 draw the samples of frame indices b, b + 1, ... (b = the frames rendered since the last other reset,
+ *                 i.e. crtc_initialize, crtc_set_scene, a commit that drops the history or a camera_changed render after
+ *                 a frame; a camera_changed render right after the commit does not reset b). Otherwise a still pixel
+ *                 would re-render the samples its history already holds, and the history would add nothing. Frames of
+ *                 camera-only epochs are unchanged. The drop-in plugin (backends/cuda) has no scene-update channel and
+ *                 does not use the option.
  *   "dynamic_scene" 0 (default) / 1: crtc_set_scene keeps on the device what crtc_update_instances / crtc_update_vertices
  *                 and crtc_commit_scene need. Takes effect at the next crtc_set_scene; with 0 nothing is kept and nothing
  *                 more runs. Every builder ("bvh_builder" 0, 1, 2). Memory: the unique geometry (12 B per unique vertex,
@@ -173,9 +190,10 @@ int crtc_update_lights(crtc_renderer *r, const crt_quad_light_t *lights, uint32_
  * commit with staged instances or vertices re-flattens every triangle (k_reflatten) and refits every node (one
  * k_bvh8_refit launch per BVH8 level). Then:
  *   - the accumulation resets as on camera_changed: accum, the AOVs and the adaptive block counts; the next frame equals
- *     frame 0 of a fresh renderer;
- *   - the denoiser's history is dropped (its reprojection assumes static geometry): crtc_read_denoise_history fails until
- *     the next crtc_denoise;
+ *     frame 0 of a fresh renderer (with option denoise_motion keeping the history: frame b of one, see the option);
+ *   - the denoiser's history is dropped (its reprojection assumes static geometry), unless option denoise_motion is on and
+ *     the commit stages no lights: then it is kept and the next crtc_denoise moves it with the geometry (step b'). Either
+ *     way crtc_read_denoise_history fails until the next crtc_denoise;
  *   - the any_far_first decision is kept; if mode 2 has not decided yet, its trial restarts as after crtc_set_scene;
  *   - frame counters and stage times do not include the commit's launches.
  * With nothing staged it does nothing: no reset, no launch. */
@@ -319,10 +337,20 @@ typedef struct crtc_denoise_params_t {
  * (I.rgb, M1, M2, n, z, nhat.xyz): integrated demodulated colour, integrated luminance moments, the samples they
  * represent, and the depth and unit normal of step 1. A call in epoch e first turns `cur` into `prev` if `cur` was written
  * in an earlier epoch, so `prev` is the output of the last call of the latest earlier epoch that had one; every call
- * overwrites `cur`. crtc_initialize and crtc_set_scene drop both. Between steps 1 and 2 above, per pixel p = (x, y):
+ * overwrites `cur`. crtc_initialize and crtc_set_scene drop both, and so does crtc_commit_scene without option
+ * denoise_motion. Between steps 1 and 2 above, per pixel p = (x, y):
  *   a. N = spp * frames accumulated (as in step 1). n_p = 0 if there is no `prev` or p's coverage is 0. Otherwise:
  *   b. d = normalize(du * ((x + 0.5) / w) + dv * ((y + 0.5) / h) + tl) with the current camera's basis (the primary ray
  *      expression at jitter 0.5), X = pos + z * d, z = p's AOV depth.
+ *   b'. Option denoise_motion, only when geometry moved (a commit with instances or vertices) since `prev` was written:
+ *      the renderer keeps, per pixel, the leaf-order triangle and barycentrics (b1, b2) of the first sample of the
+ *      epoch's first frame, in sample order, that hit geometry; with each history buffer, a copy of the instance matrices
+ *      and vertices it was written under. If p has such a record and the triangle's world vertices w0, w1, w2 now differ
+ *      (as bits) from w0', w1', w2' under prev's copy: X is replaced by X + (P' - P), P = w0 + b1 (w1 - w0) + b2 (w2 - w0)
+ *      and P' the same over w'; in step c the normal test uses s * n' in place of nhat_p, n' = the triangle's shading
+ *      normal under prev's copy, s = -1 if dot(nhat_p, n) < 0 for its current shading normal n, else 1; a non-finite
+ *      P' - P gives n_p = 0. Every other pixel (no record, or a triangle that did not move) follows b and c unchanged,
+ *      bit for bit. Without moved geometry, the option changes no bit of the output.
  *   c. (alpha, beta, gamma) = M'^-1 (X - pos') with M' = [du' | dv' | tl'] of prev's camera (inverted in double, rounded to
  *      float). Needs gamma > 0; then sx = (alpha / gamma) * w - 0.5, sy = (beta / gamma) * h - 0.5 and the 2x2 taps q
  *      around (sx, sy) get bilinear weights. A tap is valid when it is inside the image, prev's normal at q is nonzero,
