@@ -181,11 +181,13 @@ struct BinFrame {
         }
         cmin[3] = 0.f;
     }
-    // bin of the centroid on every axis: clamp((int)((c - cmin) * scale), 0, kBins - 1)
+    // bin of the centroid on every axis: clamp((int)((c - cmin) * scale), 0, kBins - 1), NaN to bin 0. A centroid or a
+    // centroid bound at +-inf (an infinite vertex, or lo + hi overflowing) makes x = inf * 0 or inf - inf; the clamp
+    // takes the bound as its first operand, so that a NaN fails both compares and becomes the bound.
     i4 bins(const Prim &p) const
     {
         f4 x = (p.centroid() - cmin) * scale;
-        x = vmin(vmax(x, splat(0.f)), splat((float)(kBins - 1)));
+        x = vmin(splat((float)(kBins - 1)), vmax(splat(0.f), x));
         return __builtin_convertvector(x, i4);
     }
 };
@@ -257,7 +259,9 @@ struct Bvh2Builder {
                     continue;
                 }
                 const float cost = acc.half_area() * cnt + right_area[b + 1] * right_cnt[b + 1];
-                if (cost < best_cost) {
+                // (a bin whose prims are all NaN on an axis keeps its reset bounds, FLT_MAX..-FLT_MAX, so a cost can be
+                // -inf or NaN; such a split would peel the range one prim at a time. Finite boxes give costs >= 0.)
+                if (cost >= 0.f && cost < best_cost) {
                     best_cost = cost;
                     best_axis = a;
                     best_bin = b;

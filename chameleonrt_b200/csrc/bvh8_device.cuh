@@ -874,9 +874,20 @@ __global__ void __launch_bounds__(kBuildBlock) k_plan_level(Lbvh b, LevelArgs lv
 
 __device__ __forceinline__ float pow2_biased(int e) { return __uint_as_float((uint32_t)e << 23); }
 
+// (int)x as x86-64 converts a double (cvttsd2si): truncation toward zero, and INT_MIN for NaN and for every x outside
+// [-2^31, 2^31). fill_node of bvh8_build.cpp converts that way; the device's own conversion saturates and maps NaN to
+// 0, which for a child box whose lower bound is +inf gives qlo = 255 where the host builder gives 0.
+__device__ __forceinline__ int double_to_int_x86(double x)
+{
+    return (x >= -2147483648.0 && x < 2147483648.0) ? (int)x : INT32_MIN;
+}
+
 // The quantisation frame of a BVH8 node over its box [blo, bhi] (fill_node of bvh8_build.cpp; k_emit_level, k_bvh8_refit
 // of scene_update.cuh): out.p = blo and the exponents out.e; step = the grid step per axis. Flat axes get a thin but
 // non-zero grid, and the far plane of the node must be representable: lo + 255 * 2^e >= hi.
+// Boxes with an infinite bound (geometry at +-inf, or a sum overflowing) take the host builder's arithmetic too: the
+// extent of an axis whose bounds are both +inf or both -inf is NaN and stays NaN through the two maxima (std::max's
+// order, which keeps its first operand when the compare fails), and the conversions are the x86 ones.
 __device__ __forceinline__ void bvh8_node_frame(const float *blo, const float *bhi, Bvh8Node &out, double *step)
 {
     float max_ext = 0.f;
@@ -885,9 +896,11 @@ __device__ __forceinline__ void bvh8_node_frame(const float *blo, const float *b
         max_ext = fmaxf(max_ext, bhi[a] - blo[a]);
     }
     for (int a = 0; a < 3; ++a) {
-        float ext = fmaxf(bhi[a] - blo[a], max_ext * (1.f / 65536.f));
-        ext = fmaxf(ext, 1e-30f);
-        int e = (int)ceil(log2((double)ext / 255.0));
+        const float thin = max_ext * (1.f / 65536.f);
+        float ext = bhi[a] - blo[a];
+        ext = ext < thin ? thin : ext;
+        ext = ext < 1e-30f ? 1e-30f : ext;
+        int e = double_to_int_x86(ceil(log2((double)ext / 255.0)));
         e = min(max(e, -100), 100);
         while (e < 100 && (double)blo[a] + 255.0 * ldexp(1.0, e) < (double)bhi[a]) {
             ++e;
@@ -903,8 +916,8 @@ __device__ __forceinline__ void bvh8_quantise_child(const Bvh8Node &out, const d
 {
     for (int a = 0; a < 3; ++a) {
         const double p = out.p[a], st = step[a];
-        int lo = (int)floor(((double)l3[a] - p) / st);
-        int hi = (int)ceil(((double)h3[a] - p) / st);
+        int lo = double_to_int_x86(floor(((double)l3[a] - p) / st));
+        int hi = double_to_int_x86(ceil(((double)h3[a] - p) / st));
         lo = min(max(lo, 0), 255);
         hi = min(max(hi, 0), 255);
         while (lo > 0 && p + lo * st > (double)l3[a]) {  // conservative: p + q*step is exact in double

@@ -156,7 +156,25 @@ int crtc_set_stream(crtc_renderer *r, void *cuda_stream);
 int crtc_initialize(crtc_renderer *r, int fb_width, int fb_height);
 
 /* RenderBackend::set_scene: flattens instances, builds the BVH8 on the host, uploads
- * geometry / materials / textures / lights, resets accumulation. */
+ * geometry / materials / textures / lights, resets accumulation.
+ * Vertex values and instance matrices are not checked: NaN, +-inf and values up to +-FLT_MAX are accepted here and by
+ * crtc_update_instances / crtc_update_vertices, by every builder (a device build that cannot progress over non-finite
+ * boxes is redone by the host builder, as "bvh_builder_fallbacks" counts). A hit is what a brute-force test of every
+ * world-space triangle with the kernel's float32 triangle formula finds: the closest t, ties to the lowest flattened id.
+ * For every ray, traces give that hit, a miss, or a hit later in (t, id) order; never a closer or a false hit. They give
+ * exactly that hit (closest hits bit for bit, occlusion answers equal) for every ray it has none for, and for every ray
+ * whose hit is well conditioned, i.e. whose triangle lies within 2^16 of its longest edges of the ray origin (farther,
+ * the triangle formula's own rounding can exceed the triangle), when:
+ *   - all world-space vertices (NaN coordinates do not count) and ray origins lie in a box of extent at most
+ *     kExactExtent = 255 * 2^46 (about 1.79e16) on each axis; or
+ *   - past that extent: every coordinate is above -kExactExtent, the hit triangle lies within 2^107, and every
+ *     direction component has magnitude at least 2^-12.
+ * Otherwise box-test planes can overflow: 2^(e+15) / |d_a| passes FLT_MAX for a node grid step 2^e with e >= 47 and a
+ * zero direction component (clamped to 1e-20), so rays straight along an axis miss a scene just wider than
+ * kExactExtent; and a node whose low corner lies below the ray origin by more than FLT_MAX * |d_a| on an axis is culled
+ * for that ray, so a single vertex at -inf or near -FLT_MAX hides every triangle that shares a node with it (in the
+ * worst case the whole scene) from every ray. Node grids stop at 2^100, so a triangle beyond about 3.2e32 from its
+ * node's low corner can be culled too. */
 int crtc_set_scene(crtc_renderer *r, const crt_scene_t *scene);
 
 /* Scene updates between frames, without a new crtc_set_scene: instances move, meshes deform, lights change. The update

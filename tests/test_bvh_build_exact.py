@@ -520,36 +520,48 @@ def assign_slots(plo, phi, clo, chi):
     return slot_child
 
 
+def _to_int_x86(x):
+    """(int)x of a float64 array as x86-64 converts it: INT_MIN for NaN and everything outside [-2^31, 2^31)."""
+    with np.errstate(invalid="ignore"):
+        return np.where((x >= -2.0**31) & (x < 2.0**31), x, -2.0**31)
+
+
 def quantise(plo, phi, clo, chi):
     """fill_node's quantisation in float64, vectorised over nodes (plo / phi: (N, 3)) and slots (clo / chi: (N, 8, 3)).
-    e is the least exponent with 255 2^e >= ext (frexp, no log2), raised until p + 255 2^e >= hi."""
+    e is the least exponent with 255 2^e >= ext (frexp, no log2), raised until p + 255 2^e >= hi. Infinite bounds follow
+    fill_node too: the extent of an axis with both bounds at the same infinity is NaN and stays NaN through its maxima
+    (std::max), and the conversions to int are x86's (a NaN or infinite ext gives e = -100 before the raise)."""
     plo, phi = plo.astype(F32), phi.astype(F32)
-    max_ext = np.fmax(F32(0), (phi - plo).max(1))
-    ext = np.fmax(phi - plo, max_ext[:, None] * F32(1.0 / 65536.0))
-    ext = np.fmax(ext, F32(1e-30)).astype(F64)
-    m, ex = np.frexp(ext)
-    e = np.where(m <= 255.0 / 256.0, ex - 8, ex - 7)
-    e = np.clip(e, -100, 100)
-    while True:
-        up = (e < 100) & (plo.astype(F64) + 255.0 * np.ldexp(1.0, e) < phi.astype(F64))
-        if not up.any():
-            break
-        e = e + up
-    st = np.ldexp(1.0, e)[:, None, :]
-    p = plo.astype(F64)[:, None, :]
-    lo = np.floor((clo.astype(F64) - p) / st)
-    hi = np.ceil((chi.astype(F64) - p) / st)
+    with np.errstate(invalid="ignore", over="ignore"):
+        d = phi - plo
+        max_ext = np.fmax(F32(0), np.fmax.reduce(d, 1))
+        thin = max_ext[:, None] * F32(1.0 / 65536.0)
+        ext = np.where(d < thin, thin, d)
+        ext = np.where(ext < F32(1e-30), F32(1e-30), ext).astype(F64)
+        m, ex = np.frexp(ext)
+        e = np.where(np.isfinite(ext), np.where(m <= 255.0 / 256.0, ex - 8, ex - 7), -100)
+        e = np.clip(e, -100, 100)
+        while True:
+            up = (e < 100) & (plo.astype(F64) + 255.0 * np.ldexp(1.0, e) < phi.astype(F64))
+            if not up.any():
+                break
+            e = e + up
+        st = np.ldexp(1.0, e)[:, None, :]
+        p = plo.astype(F64)[:, None, :]
+        lo = _to_int_x86(np.floor((clo.astype(F64) - p) / st))
+        hi = _to_int_x86(np.ceil((chi.astype(F64) - p) / st))
     lo, hi = np.clip(lo, 0, 255), np.clip(hi, 0, 255)
-    while True:
-        dn = (lo > 0) & (p + lo * st > clo)
-        if not dn.any():
-            break
-        lo -= dn
-    while True:
-        upm = (hi < 255) & (p + hi * st < chi)
-        if not upm.any():
-            break
-        hi += upm
+    with np.errstate(invalid="ignore"):
+        while True:
+            dn = (lo > 0) & (p + lo * st > clo)
+            if not dn.any():
+                break
+            lo -= dn
+        while True:
+            upm = (hi < 255) & (p + hi * st < chi)
+            if not upm.any():
+                break
+            hi += upm
     flat = hi <= lo
     hi = np.where(flat & (hi < 255), lo + 1, hi)
     lo = np.where(flat & ~(hi < 255), hi - 1, lo)
