@@ -38,6 +38,7 @@ C_ABI_SYMBOLS = (
     "crtc_local_buffers", "crtc_assemble_rank", "crtc_export_frame", "crtc_import_frame", "crtc_share_frame", "crtc_read_img", "crtc_frame_wait", "crtc_copy_img_to_array",
     "crtc_read_aov", "crtc_denoise", "crtc_read_denoise_history", "crtc_set_adaptive", "crtc_read_adaptive",
     "crtc_update_instances", "crtc_update_vertices", "crtc_update_lights", "crtc_commit_scene",
+    "crtc_render_views", "crtc_read_view",
 )
 # Per-pixel layout of crtc_read_aov: name -> (first float, number of floats)
 AOV_LAYOUT = {"albedo": (0, 3), "coverage": (3, 1), "normal": (4, 3), "depth": (7, 1), "lum_m1": (8, 1), "lum_m2": (9, 1)}
@@ -56,6 +57,12 @@ class CDenoiseParams(C.Structure):
 class CAdaptiveParams(C.Structure):
     """crtc_adaptive_params_t"""
     _fields_ = [("threshold", C.c_float), ("min_frames", C.c_uint32), ("max_frames", C.c_uint32)]
+
+
+class CView(C.Structure):
+    """crtc_view_t"""
+    _fields_ = [("pos", C.c_float * 3), ("dir", C.c_float * 3), ("up", C.c_float * 3), ("fovy", C.c_float),
+                ("camera_changed", C.c_int)]
 
 
 def lib_path() -> str:
@@ -110,6 +117,8 @@ def load_lib() -> C.CDLL:
     lib.crtc_update_vertices.argtypes = [vp, C.c_uint32, C.c_uint32, vp, C.c_uint32]
     lib.crtc_update_lights.argtypes = [vp, vp, C.c_uint32]
     lib.crtc_commit_scene.argtypes = [vp]
+    lib.crtc_render_views.argtypes = [vp, C.POINTER(CView), C.c_uint32, C.c_uint32]
+    lib.crtc_read_view.argtypes = [vp, C.c_uint32, vp, vp]
     _lib = lib
     return lib
 
@@ -126,7 +135,7 @@ class RenderCUDA:
                  count_traversal: bool = False, bvh_threads: int = 0, stream: Optional[int] = None,
                  any_far_first: Optional[int] = None, bvh_builder: Optional[str] = None,
                  tri_pass_defer: Optional[int] = None, shade_sort: Optional[int] = None, aov: bool = False,
-                 denoise_history: int = 0, dynamic_scene: bool = False, denoise_motion: bool = False):
+                 denoise_history: int = 0, dynamic_scene: bool = False, denoise_motion: bool = False, views: int = 1):
         self.lib = load_lib()
         self.h = C.c_void_p()
         self._check(self.lib.crtc_create(C.byref(self.h), device))
@@ -170,6 +179,8 @@ class RenderCUDA:
             self._check(self.lib.crtc_set_option(self.h, b"dynamic_scene", 1))
         if denoise_motion:  # commit_scene keeps denoise()'s history, moved with the geometry (option "denoise_motion")
             self._check(self.lib.crtc_set_option(self.h, b"denoise_motion", 1))
+        if views != 1:  # cameras render_views traces together (option "views")
+            self._check(self.lib.crtc_set_option(self.h, b"views", int(views)))
         if stream is not None:
             self._check(self.lib.crtc_set_stream(self.h, C.c_void_p(stream)))
         self.width = self.height = 0
@@ -256,6 +267,31 @@ class RenderCUDA:
         _u, up_ = _vec3(up)
         self._check(self.lib.crtc_render_async(self.h, pp, dp, up_, C.c_float(fovy), 1 if camera_changed else 0,
                                                num_frames))
+
+    # ---- multi-view rendering (include/crt_cuda.h: crtc_render_views) ----
+    def render_views(self, cameras, camera_changed=True, num_frames: int = 1) -> None:
+        """Enqueues ``num_frames`` frames of every camera as one wavefront (needs ``views=len(cameras)``); returns
+        immediately, ``sync()`` collects it. A camera is ``(pos, dir, up, fovy)`` or a dict with ``position`` (or ``eye``),
+        ``center``, ``up`` and ``fov_y``, like ``scene_io.load_scene(path).cameras``. ``camera_changed``: one bool for
+        every view or one per view. View k ends bit-identical to a one-view renderer given the same render_async calls."""
+        from .camera import view_args
+
+        n = len(cameras)
+        flags = [bool(camera_changed)] * n if isinstance(camera_changed, (bool, int)) else [bool(c) for c in camera_changed]
+        if len(flags) != n:
+            raise ValueError("camera_changed: one flag per camera")
+        arr = (CView * max(1, n))()
+        for k, cam in enumerate(cameras):
+            pos, d, up, fovy = view_args(cam)
+            arr[k] = CView((C.c_float * 3)(*pos), (C.c_float * 3)(*d), (C.c_float * 3)(*up), float(fovy), int(flags[k]))
+        self._check(self.lib.crtc_render_views(self.h, arr, n, int(num_frames)))
+
+    def read_view(self, k: int):
+        """View ``k`` of a multi-view renderer (crtc_read_view): (rgb (h, w, 3) float32, img (h, w) uint32 RGBA8)."""
+        rgb = np.zeros((self.height, self.width, 3), dtype=np.float32)
+        img = np.zeros((self.height, self.width), dtype=np.uint32)
+        self._check(self.lib.crtc_read_view(self.h, int(k), rgb.ctypes.data, img.ctypes.data))
+        return rgb, img
 
     def set_stream(self, cuda_stream: Optional[int]) -> None:
         """crtc_set_stream: the CUDA stream (a cudaStream_t as an integer) every later launch and copy of this renderer

@@ -38,3 +38,14 @@ class ArcballCamera:
 
     def center(self):
         return self._center.copy()
+
+
+def view_args(cam):
+    """``(pos, dir, up, fovy)`` for ``RenderCUDA.render``: ``cam`` is that tuple already, or a camera dict with ``position``
+    (``.crts`` cameras, ``scene_io``) or ``eye`` (``scenes``), ``center``, ``up`` and ``fov_y``, seen through
+    ``ArcballCamera`` as the reference app does."""
+    if isinstance(cam, dict):
+        c = ArcballCamera(cam["position"] if "position" in cam else cam["eye"], cam["center"], cam["up"])
+        return c.eye(), c.dir(), c.up(), float(cam["fov_y"])
+    pos, d, up, fovy = cam
+    return pos, d, up, float(fovy)

@@ -145,6 +145,19 @@ struct crtc_renderer {
     uint32_t spp = 1;
     bool have_scene = false;
 
+    // Option "views" (crtc_render_views): `views` is the option, `views_active` what the last crtc_initialize set up. With
+    // views_active > 1 the local and full framebuffers hold that many views, view-major, and view k's frame counter is
+    // view_frames[k] (frame_id is then unused).
+    uint32_t views = 1, views_active = 1;
+    std::vector<uint32_t> view_frames{0u};
+    void require_single_view(const char *what) const
+    {
+        if (views_active > 1) {
+            throw std::runtime_error(std::string(what) + ": this renderer was initialized with option views = " +
+                                     std::to_string(views_active) + "; render with crtc_render_views and read with crtc_read_view");
+        }
+    }
+
     // device scene
     DeviceBuffer<float4> d_nodes, d_tris, d_shade, d_materials, d_lights;
     DeviceBuffer<uint32_t> d_texels;
@@ -285,6 +298,10 @@ struct crtc_renderer {
         if (!params) {
             adaptive = false;
             return;
+        }
+        if (views_active > 1) {
+            throw std::runtime_error("crtc_set_adaptive: adaptive sampling is not available with crtc_render_views; this renderer "
+                                     "was initialized with option views = " + std::to_string(views_active));
         }
         if (aov_active) {
             throw std::runtime_error("crtc_set_adaptive: adaptive sampling cannot be combined with option aov (the AOVs and the "
@@ -685,6 +702,18 @@ struct crtc_renderer {
                                      "denoiser assume the same number of samples in every pixel); turn it off with "
                                      "crtc_set_adaptive(r, NULL) first");
         }
+        if (views > 1) {
+            const std::string v = "initialize: option views = " + std::to_string(views) + " (crtc_render_views) ";
+            if (aov) {
+                throw std::runtime_error(v + "cannot be combined with option aov (AOVs and the denoiser have one view)");
+            }
+            if (world_size > 1) {
+                throw std::runtime_error(v + "needs the whole frame on one renderer (world_size 1)");
+            }
+            if (adaptive) {
+                throw std::runtime_error(v + "cannot be combined with adaptive sampling; turn it off with crtc_set_adaptive(r, NULL) first");
+            }
+        }
         make_current();
         CUDA_CHECK(cudaStreamSynchronize(stream));
         unpin_img();             // (the caller's img buffer is reallocated with the new size)
@@ -692,6 +721,8 @@ struct crtc_renderer {
         frame_exported = false;  // crtc_export_frame / crtc_import_frame must be called again
         frame_id = 0;
         sample_base = 0;
+        views_active = views;
+        view_frames.assign(views, 0u);
         fb_w = w;
         fb_h = h;
         ntx = crt::tiles_along(w);
@@ -699,16 +730,17 @@ struct crtc_renderer {
         npx_local = (uint32_t)local_tiles.size() * crt::kTilePixels;
         assemble_tiles.clear();
         d_tile_ids.upload(local_tiles.data(), local_tiles.size(), stream);
-        d_accum_local.alloc((size_t)npx_local * 3);
-        d_img_local.alloc(npx_local);
-        d_accum_full.alloc((size_t)w * h * 3);
-        d_img_full.alloc((size_t)w * h + crt::kSyncWords);  // + the frame completion flags (kernels.cuh)
+        const size_t nv = views_active;
+        d_accum_local.alloc((size_t)npx_local * 3 * nv);
+        d_img_local.alloc(npx_local * nv);
+        d_accum_full.alloc((size_t)w * h * 3 * nv);
+        d_img_full.alloc((size_t)w * h * nv + crt::kSyncWords);  // + the frame completion flags (kernels.cuh)
         if (npx_local) {
-            CUDA_CHECK(cudaMemsetAsync(d_accum_local.ptr, 0, (size_t)npx_local * 3 * sizeof(float), stream));
-            CUDA_CHECK(cudaMemsetAsync(d_img_local.ptr, 0, (size_t)npx_local * 4, stream));
+            CUDA_CHECK(cudaMemsetAsync(d_accum_local.ptr, 0, (size_t)npx_local * 3 * nv * sizeof(float), stream));
+            CUDA_CHECK(cudaMemsetAsync(d_img_local.ptr, 0, (size_t)npx_local * nv * 4, stream));
         }
-        CUDA_CHECK(cudaMemsetAsync(d_accum_full.ptr, 0, (size_t)w * h * 3 * sizeof(float), stream));
-        CUDA_CHECK(cudaMemsetAsync(d_img_full.ptr, 0, ((size_t)w * h + crt::kSyncWords) * 4, stream));
+        CUDA_CHECK(cudaMemsetAsync(d_accum_full.ptr, 0, (size_t)w * h * 3 * nv * sizeof(float), stream));
+        CUDA_CHECK(cudaMemsetAsync(d_img_full.ptr, 0, ((size_t)w * h * nv + crt::kSyncWords) * 4, stream));
         aov_active = aov;
         dn_history_active = dn_history;
         dn_motion_active = dn_motion;
@@ -828,8 +860,9 @@ struct crtc_renderer {
             scene_info[6 + i] = phase_ms[i];
         }
         scene_info[11] = (bvh_builder == 1 && built_on_device) ? (double)build_rounds : 0.0;
+        view_frames.assign(views_active, 0u);
         if (npx_local) {
-            CUDA_CHECK(cudaMemsetAsync(d_accum_local.ptr, 0, (size_t)npx_local * 3 * sizeof(float), stream));
+            CUDA_CHECK(cudaMemsetAsync(d_accum_local.ptr, 0, (size_t)npx_local * 3 * views_active * sizeof(float), stream));
             if (aov_active) {
                 CUDA_CHECK(cudaMemsetAsync(aov_state.local.ptr, 0, (size_t)npx_local * crt::kAovFloats * sizeof(float), stream));
             }
@@ -896,6 +929,7 @@ struct crtc_renderer {
             sample_base += frame_id;
         }
         frame_id = 0;  // as camera_changed: accum, AOVs and the adaptive block counts restart
+        view_frames.assign(views_active, 0u);
         adaptive_epoch = false;
         if (!auto_decided) {
             auto_frames = 0;  // an undecided any_far_first trial restarts
@@ -940,15 +974,7 @@ struct crtc_renderer {
         crt::FrameLayout fl = frame_layout();
         fl.frames = num_frames;
         const crt::PathState ps = path_state();
-        if (record_pool.empty()) {
-            record_pool.emplace_back(new FrameRecord());
-        }
-        in_flight.push_back(std::move(record_pool.back()));
-        record_pool.pop_back();
-        FrameRecord &rec = *in_flight.back();
-        rec.num_events = 0;
-        rec.launches = 0;
-        rec.all_stages = stage_events || (any_far_first == 2 && !auto_decided);  // (the shadow-order trial reads the traversal stage)
+        FrameRecord &rec = new_record();
 
         const bool shared_dst = frame_exported && world_size > 1, shared_src = peer_accum_full != nullptr && !frame_exported;
         if (shared_dst || shared_src) {
@@ -959,10 +985,7 @@ struct crtc_renderer {
             // starting the next wavefront: the assembling rank is done with the previous frame, peers may overwrite it
             crt::k_set_word<<<1, 32, 0, stream>>>(sync_words() + crt::kSyncConsumed, share_seq);
         }
-        CUDA_CHECK(cudaMemsetAsync(d_counters.ptr, 0, crt::kNumCounters * sizeof(uint32_t), stream));
-        if (count_traversal) {
-            CUDA_CHECK(cudaMemsetAsync(d_trav_counters.ptr, 0, 4 * sizeof(unsigned long long), stream));
-        }
+        zero_counters();
         // adaptive sampling: which blocks render how many of this wavefront's frames, decided once per call
         const bool adaptive_frame = adaptive || adaptive_epoch;
         crt::AdaptiveSelect sel{};
@@ -986,12 +1009,6 @@ struct crtc_renderer {
         const crt::AdaptiveFrame ad = adaptive_state.frame(adaptive_base);
         if (npaths) {
             const unsigned g256 = (unsigned)((npaths + 255) / 256);
-            // k_nee_resolve strides over its queue: two waves of resident blocks cover any queue length
-            if (num_sms == 0) {
-                CUDA_CHECK(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, device));
-            }
-            const unsigned g128 = (unsigned)((npaths + 127) / 128);
-            const unsigned g_nee = (unsigned)std::min<size_t>((npaths + 255) / 256, (size_t)num_sms * 8 * 2);
             if (adaptive_frame) {  // (its time counts as raygen)
                 adaptive_state.select(fl, sel, stream);
                 rec.launches += 1;
@@ -1000,11 +1017,7 @@ struct crtc_renderer {
                 crt::k_raygen<<<g256, 256, 0, stream>>>(view, fl, ps);
             }
             rec.mark(stream, kStRaygen);
-            // closest hit of the primary rays, then per bounce: shade -> one traversal launch for this
-            // bounce's shadow rays AND the next bounce's continuation rays -> NEE resolve
-            launch_traverse(sc, ps, ps.queue[0], ps.counters + crt::kCntQueue, nullptr, ps.counters + crt::kCntWork);
-            rec.mark(stream, kStPrimary);
-            rec.launches += 2;
+            launch_primary(sc, ps, rec);
             if (aov_active) {  // (its time counts as shading: the next mark closes the stage)
                 aov_state.launch_primary(sc, fl, ps, frame_id, stream);
                 rec.launches += 1;
@@ -1013,28 +1026,7 @@ struct crtc_renderer {
                     rec.launches += 1;
                 }
             }
-            for (int b = 0; b < max_depth; ++b) {
-                const uint32_t *qin = ps.queue[b & 1];
-                uint32_t *qout = ps.queue[(b + 1) & 1];
-                if (shade_sort == 2 || (shade_sort == 1 && b > 0)) {
-                    // (its time counts as shading: the next mark closes the stage)
-                    rec.launches += sort_shade_queue(sc, ps, qin, b, npaths);
-                    qin = d_queue_sorted.ptr;
-                }
-                if (sc.tex_objects) {
-                    crt::k_shade<true><<<g128, 128, 0, stream>>>(sc, ps, qin, qout, b, max_depth);
-                } else {
-                    crt::k_shade<false><<<g128, 128, 0, stream>>>(sc, ps, qin, qout, b, max_depth);
-                }
-                rec.mark(stream, kStShade);
-                const bool last = b + 1 == max_depth;
-                launch_traverse(sc, ps, qout, last ? nullptr : ps.counters + crt::kCntQueue + b + 1,
-                                ps.counters + crt::kCntShadow + b, ps.counters + crt::kCntWork + 1 + b);
-                rec.mark(stream, kStTraverse);
-                crt::k_nee_resolve<<<g_nee, 256, 0, stream>>>(ps, qin, b);
-                rec.mark(stream, kStNee);
-                rec.launches += 3;
-            }
+            launch_bounces(sc, ps, npaths, rec);
             const unsigned gpx = (unsigned)((npx_local + 255) / 256);
             // where the resolved pixels also go as a full row-major frame: this renderer's own full frame (single
             // GPU, or the assembling rank of a peer-written frame), the assembling rank's full frame over NVLink
@@ -1072,6 +1064,77 @@ struct crtc_renderer {
             // a rank that owns no tile of this frame (more ranks than tiles) still has to say "done"
             crt::k_set_word<<<1, 32, 0, stream>>>(peer_sync_words() + rank, share_seq + 1u);
         }
+        finish_record(rec, num_frames);
+        frame_id += num_frames;
+        if (shared_dst || shared_src) {
+            ++share_seq;
+        }
+        return rec;
+    }
+
+    // ---- the parts of a wavefront that do not depend on its cameras (enqueue_frame, enqueue_views) ----
+    FrameRecord &new_record()
+    {
+        if (record_pool.empty()) {
+            record_pool.emplace_back(new FrameRecord());
+        }
+        in_flight.push_back(std::move(record_pool.back()));
+        record_pool.pop_back();
+        FrameRecord &rec = *in_flight.back();
+        rec.num_events = 0;
+        rec.launches = 0;
+        rec.all_stages = stage_events || (any_far_first == 2 && !auto_decided);  // (the shadow-order trial reads the traversal stage)
+        return rec;
+    }
+    void zero_counters()
+    {
+        CUDA_CHECK(cudaMemsetAsync(d_counters.ptr, 0, crt::kNumCounters * sizeof(uint32_t), stream));
+        if (count_traversal) {
+            CUDA_CHECK(cudaMemsetAsync(d_trav_counters.ptr, 0, 4 * sizeof(unsigned long long), stream));
+        }
+    }
+    // closest hit of the primary rays (the raygen launch is counted here too)
+    void launch_primary(const crt::DeviceScene &sc, const crt::PathState &ps, FrameRecord &rec)
+    {
+        launch_traverse(sc, ps, ps.queue[0], ps.counters + crt::kCntQueue, nullptr, ps.counters + crt::kCntWork);
+        rec.mark(stream, kStPrimary);
+        rec.launches += 2;
+    }
+    // per bounce: shade -> one traversal launch for this bounce's shadow rays AND the next bounce's continuation rays
+    // -> NEE resolve
+    void launch_bounces(const crt::DeviceScene &sc, const crt::PathState &ps, size_t npaths, FrameRecord &rec)
+    {
+        // k_nee_resolve strides over its queue: two waves of resident blocks cover any queue length
+        if (num_sms == 0) {
+            CUDA_CHECK(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, device));
+        }
+        const unsigned g128 = (unsigned)((npaths + 127) / 128);
+        const unsigned g_nee = (unsigned)std::min<size_t>((npaths + 255) / 256, (size_t)num_sms * 8 * 2);
+        for (int b = 0; b < max_depth; ++b) {
+            const uint32_t *qin = ps.queue[b & 1];
+            uint32_t *qout = ps.queue[(b + 1) & 1];
+            if (shade_sort == 2 || (shade_sort == 1 && b > 0)) {
+                // (its time counts as shading: the next mark closes the stage)
+                rec.launches += sort_shade_queue(sc, ps, qin, b, npaths);
+                qin = d_queue_sorted.ptr;
+            }
+            if (sc.tex_objects) {
+                crt::k_shade<true><<<g128, 128, 0, stream>>>(sc, ps, qin, qout, b, max_depth);
+            } else {
+                crt::k_shade<false><<<g128, 128, 0, stream>>>(sc, ps, qin, qout, b, max_depth);
+            }
+            rec.mark(stream, kStShade);
+            const bool last = b + 1 == max_depth;
+            launch_traverse(sc, ps, qout, last ? nullptr : ps.counters + crt::kCntQueue + b + 1,
+                            ps.counters + crt::kCntShadow + b, ps.counters + crt::kCntWork + 1 + b);
+            rec.mark(stream, kStTraverse);
+            crt::k_nee_resolve<<<g_nee, 256, 0, stream>>>(ps, qin, b);
+            rec.mark(stream, kStNee);
+            rec.launches += 3;
+        }
+    }
+    void finish_record(FrameRecord &rec, uint32_t num_frames)
+    {
         CUDA_CHECK(cudaMemcpyAsync(rec.h_counters, d_counters.ptr, crt::kNumCounters * sizeof(uint32_t),
                                    cudaMemcpyDeviceToHost, stream));
         if (count_traversal) {
@@ -1079,12 +1142,89 @@ struct crtc_renderer {
                                        cudaMemcpyDeviceToHost, stream));
         }
         CUDA_CHECK(cudaGetLastError());
-        frame_id += num_frames;
         rec.frames = num_frames;
-        if (shared_dst || shared_src) {
-            ++share_seq;
+    }
+
+    // crtc_render_views: `num_frames` frames of every view as ONE wavefront (kernels.cuh: k_raygen_views, k_resolve_views);
+    // view k is seeded and folded with its own frame counter, so it ends bit-identical to a one-view renderer's frame.
+    // With one view this is crtc_render_async.
+    void enqueue_views(const crtc_view_t *vs, uint32_t num_views, uint32_t num_frames)
+    {
+        if (!vs) {
+            throw std::runtime_error("crtc_render_views: views is NULL");
         }
-        return rec;
+        if (num_views != views_active) {
+            throw std::runtime_error("crtc_render_views: num_views = " + std::to_string(num_views) + " differs from option views = " +
+                                     std::to_string(views_active) + " of the last crtc_initialize");
+        }
+        if (views_active == 1) {
+            enqueue_frame(vs[0].pos, vs[0].dir, vs[0].up, vs[0].fovy, vs[0].camera_changed != 0, num_frames);
+            return;
+        }
+        if (num_frames < 1 || num_frames > 64) {
+            throw std::runtime_error("crtc_render_views: num_frames must be in [1, 64]");
+        }
+        if (!have_scene) {
+            throw std::runtime_error("crtc_render_views: set_scene() has not been called");
+        }
+        const size_t npaths = (size_t)npx_local * spp * num_frames * num_views;
+        if (npaths >= 0x7fffffffull) {
+            throw std::runtime_error("crtc_render_views: more than 2^31 paths in flight on one device (views x num_frames x spp x "
+                                     "64x64-padded pixels)");
+        }
+        make_current();
+        crt::ViewTable table{};
+        table.num_views = num_views;
+        for (uint32_t k = 0; k < num_views; ++k) {
+            if (vs[k].camera_changed) {
+                view_frames[k] = 0;
+            }
+            table.view[k] = crt::make_view_params(vs[k].pos, vs[k].dir, vs[k].up, vs[k].fovy, fb_w, fb_h, view_frames[k]);
+        }
+        ensure_path_buffers(npaths);
+        frame_far_first = pick_far_first(false);
+        const crt::DeviceScene sc = device_scene();
+        crt::FrameLayout fl = frame_layout();
+        fl.frames = num_frames;
+        const crt::PathState ps = path_state();
+        FrameRecord &rec = new_record();
+        rec.mark(stream, -1);
+        zero_counters();
+        crt_host::launch(crt::k_raygen_views, (unsigned)((npaths + 255) / 256), 256, stream, table, fl, ps);
+        rec.mark(stream, kStRaygen);
+        launch_primary(sc, ps, rec);
+        launch_bounces(sc, ps, npaths, rec);
+        crt_host::launch(crt::k_resolve_views, (unsigned)(((size_t)npx_local * num_views + 255) / 256), 256, stream, table, fl, ps,
+                         d_accum_local.ptr, d_img_local.ptr, d_accum_full.ptr, d_img_full.ptr);
+        rec.launches += 1;
+        rec.mark(stream, kStResolve);
+        finish_record(rec, num_frames);
+        for (uint32_t k = 0; k < num_views; ++k) {
+            view_frames[k] += num_frames;
+        }
+    }
+
+    void read_view(uint32_t view, float *rgb_out, uint32_t *img_out)
+    {
+        if (fb_w == 0) {
+            throw std::runtime_error("crtc_read_view: initialize() has not been called");
+        }
+        if (view >= views_active) {
+            throw std::runtime_error("crtc_read_view: view " + std::to_string(view) + " is out of range (option views = " +
+                                     std::to_string(views_active) + " at the last crtc_initialize)");
+        }
+        make_current();
+        frame_wait();  // (a shared one-view frame: every rank's tiles first; no-op otherwise)
+        const size_t n = (size_t)fb_w * fb_h;
+        if (rgb_out) {
+            CUDA_CHECK(cudaMemcpyAsync(rgb_out, d_accum_full.ptr + view * n * 3, n * 3 * sizeof(float), cudaMemcpyDeviceToHost, stream));
+        }
+        if (img_out) {
+            CUDA_CHECK(cudaMemcpyAsync(img_out, d_img_full.ptr + view * n, n * 4, cudaMemcpyDeviceToHost, stream));
+        }
+        CUDA_CHECK(cudaStreamSynchronize(stream));
+        CUDA_CHECK(cudaGetLastError());
+        check_sync_error();
     }
 
     // After a stream synchronisation: folds every in-flight frame's events and counters into
@@ -1572,6 +1712,11 @@ int crtc_set_option(crtc_renderer *r, const char *key, int64_t value)
             r->dynamic_scene = value != 0;  // takes effect at the next crtc_set_scene
         } else if (k == "aov") {
             r->aov = value != 0;  // takes effect at the next crtc_initialize
+        } else if (k == "views") {
+            if (value < 1 || value > crt::kMaxViews) {
+                throw std::runtime_error("views must be in [1, 64]");
+            }
+            r->views = (uint32_t)value;  // takes effect at the next crtc_initialize
         } else if (k == "denoise_history") {
             if (value < 0 || value > 1024) {
                 throw std::runtime_error("denoise_history must be in [0, 1024] (0 = off)");
@@ -1631,6 +1776,8 @@ int crtc_get_option(crtc_renderer *r, const char *key, int64_t *value)
             *value = r->dynamic_scene ? 1 : 0;
         } else if (k == "aov") {
             *value = r->aov ? 1 : 0;
+        } else if (k == "views") {
+            *value = r->views;
         } else if (k == "denoise_history") {
             *value = r->dn_history;
         } else if (k == "denoise_motion") {
@@ -1696,13 +1843,23 @@ int crtc_commit_scene(crtc_renderer *r)
 int crtc_render(crtc_renderer *r, const float *pos, const float *dir, const float *up, float fovy, int camera_changed,
                 int readback_framebuffer, uint32_t *img, crt_render_stats_t *stats)
 {
-    CRTC_TRY({ require_renderer(r); r->render(pos, dir, up, fovy, camera_changed != 0, readback_framebuffer != 0, img, stats); })
+    CRTC_TRY({ require_renderer(r); r->require_single_view("crtc_render"); r->render(pos, dir, up, fovy, camera_changed != 0, readback_framebuffer != 0, img, stats); })
 }
 
 int crtc_render_async(crtc_renderer *r, const float *pos, const float *dir, const float *up, float fovy,
                       int camera_changed, uint32_t num_frames)
 {
-    CRTC_TRY({ require_renderer(r); r->enqueue_frame(pos, dir, up, fovy, camera_changed != 0, num_frames); })
+    CRTC_TRY({ require_renderer(r); r->require_single_view("crtc_render_async"); r->enqueue_frame(pos, dir, up, fovy, camera_changed != 0, num_frames); })
+}
+
+int crtc_render_views(crtc_renderer *r, const crtc_view_t *views, uint32_t num_views, uint32_t num_frames)
+{
+    CRTC_TRY({ require_renderer(r); r->enqueue_views(views, num_views, num_frames); })
+}
+
+int crtc_read_view(crtc_renderer *r, uint32_t view, float *rgb_out, uint32_t *img_out)
+{
+    CRTC_TRY({ require_renderer(r); r->read_view(view, rgb_out, img_out); })
 }
 
 int crtc_sync(crtc_renderer *r, crt_render_stats_t *total, float *stage_ms_sum, uint64_t *counters_sum,
@@ -1719,6 +1876,7 @@ int crtc_sync(crtc_renderer *r, crt_render_stats_t *total, float *stage_ms_sum, 
 int crtc_read_accum(crtc_renderer *r, float *rgb_out)
 {
     CRTC_TRY({ require_renderer(r);
+        r->require_single_view("crtc_read_accum");
         r->make_current();
         r->frame_wait();
         CUDA_CHECK(cudaMemcpyAsync(rgb_out, r->d_accum_full.ptr, (size_t)r->fb_w * r->fb_h * 3 * sizeof(float),
@@ -1731,6 +1889,7 @@ int crtc_read_accum(crtc_renderer *r, float *rgb_out)
 int crtc_read_img(crtc_renderer *r, uint32_t *img)
 {
     CRTC_TRY({ require_renderer(r);
+        r->require_single_view("crtc_read_img");
         r->make_current();
         r->frame_wait();  // (a shared frame: every rank's tiles first; no-op otherwise)
         if (img == r->pinned_img || r->pin_repeated_reads) {  // (a caller that reads into the same buffer every frame)
@@ -1832,6 +1991,7 @@ int crtc_bench_trace(crtc_renderer *r, const float *rays_host, uint64_t n, int a
 int crtc_local_buffers(crtc_renderer *r, void **accum_dev, void **img_dev, uint32_t *num_local_tiles)
 {
     CRTC_TRY({ require_renderer(r);
+        r->require_single_view("crtc_local_buffers");
         *accum_dev = r->d_accum_local.ptr;
         *img_dev = r->d_img_local.ptr;
         *num_local_tiles = (uint32_t)r->local_tiles.size();
@@ -1840,7 +2000,7 @@ int crtc_local_buffers(crtc_renderer *r, void **accum_dev, void **img_dev, uint3
 
 int crtc_assemble_rank(crtc_renderer *r, int src_rank, int world_size, const void *accum_dev, const void *img_dev)
 {
-    CRTC_TRY({ require_renderer(r); r->assemble_rank(src_rank, world_size, accum_dev, img_dev); })
+    CRTC_TRY({ require_renderer(r); r->require_single_view("crtc_assemble_rank"); r->assemble_rank(src_rank, world_size, accum_dev, img_dev); })
 }
 
 int crtc_export_frame(crtc_renderer *r, void *handles_out)
@@ -1849,13 +2009,14 @@ int crtc_export_frame(crtc_renderer *r, void *handles_out)
         if (!handles_out) {
             throw std::runtime_error("crtc_export_frame: null output");
         }
+        r->require_single_view("crtc_export_frame");
         r->export_frame(handles_out);
     })
 }
 
 int crtc_import_frame(crtc_renderer *r, const void *handles)
 {
-    CRTC_TRY({ require_renderer(r); r->import_frame(handles); })
+    CRTC_TRY({ require_renderer(r); r->require_single_view("crtc_import_frame"); r->import_frame(handles); })
 }
 
 int crtc_copy_img_to_array(crtc_renderer *r, void *cuda_array)
@@ -1864,6 +2025,7 @@ int crtc_copy_img_to_array(crtc_renderer *r, void *cuda_array)
         if (!cuda_array) {
             throw std::runtime_error("crtc_copy_img_to_array: array is NULL");
         }
+        r->require_single_view("crtc_copy_img_to_array");
         r->make_current();
         r->frame_wait();
         CUDA_CHECK(cudaMemcpy2DToArrayAsync(static_cast<cudaArray_t>(cuda_array), 0, 0, r->d_img_full.ptr, (size_t)r->fb_w * 4,
@@ -1884,6 +2046,8 @@ int crtc_share_frame(crtc_renderer *dst, crtc_renderer *src)
         if (!dst || !src) {
             throw std::runtime_error("crtc_share_frame: null renderer");
         }
+        dst->require_single_view("crtc_share_frame");
+        src->require_single_view("crtc_share_frame");
         src->share_frame_of(dst);
     })
 }

@@ -211,6 +211,49 @@ __global__ void __launch_bounds__(256) k_raygen(ViewParams view, FrameLayout f, 
 }
 
 // ---------------------------------------------------------------------------------------
+// Multi-view wavefronts (crtc_render_views): the F frames of V cameras traced together. Path i = lp + s * (V * npx_local),
+// local pixel lp = v * npx_local + lp_v of view v; npx_local is a multiple of 4096, so a warp never straddles two views.
+// The table is a kernel parameter (64 x 52 B, within CUDA 12.1's 32 KB limit): no upload, no synchronisation.
+// view[v].frame_id = b_v, the frames view v has accumulated since its last reset.
+constexpr uint32_t kMaxViews = 64;
+struct ViewTable {
+    ViewParams view[kMaxViews];
+    uint32_t num_views;
+};
+
+// k_raygen for every view of the table: path (v, lp_v, s) is seeded as k_raygen seeds sample s of pixel lp_v for view v's
+// camera and frame b_v, so that each view's paths are those of a one-view wavefront.
+__global__ void __launch_bounds__(256) k_raygen_views(const __grid_constant__ ViewTable views, FrameLayout f, PathState ps)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t npx_all = f.npx_local * views.num_views;
+    const uint32_t npaths = npx_all * f.spp * f.frames;
+    bool valid = false;
+    if (i < npaths) {
+        const uint32_t lp = i % npx_all, s = i / npx_all;
+        const ViewParams &view = views.view[lp / f.npx_local];
+        uint32_t x, y;
+        if (local_pixel_coords(f, lp % f.npx_local, x, y)) {
+            valid = true;
+            uint32_t rng = get_rng(x + y * (uint32_t)f.fb_w, view.frame_id * f.spp + 1u + s);
+            const float px_x = ((float)x + lcg_randomf(rng)) / (float)(uint32_t)f.fb_w;
+            const float px_y = ((float)y + lcg_randomf(rng)) / (float)(uint32_t)f.fb_h;
+            const float3 dir = normalize(mk3(view.dir_du.x * px_x + view.dir_dv.x * px_y + view.dir_top_left.x,
+                                             view.dir_du.y * px_x + view.dir_dv.y * px_y + view.dir_top_left.y,
+                                             view.dir_du.z * px_x + view.dir_dv.z * px_y + view.dir_top_left.z));
+            ps.ray_o[i] = make_float4(view.pos.x, view.pos.y, view.pos.z, 0.f);
+            ps.ray_d[i] = make_float4(dir.x, dir.y, dir.z, 1e20f);
+            ps.thr_rng[i] = make_float4(1.f, 1.f, 1.f, __uint_as_float(rng));
+            ps.radiance[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+    }
+    const uint32_t idx = warp_append(ps.counters + kCntQueue, valid);
+    if (valid) {
+        ps.queue[0][idx] = i;
+    }
+}
+
+// ---------------------------------------------------------------------------------------
 // Traversal kernels: persistent warps with dynamic ray fetch.
 //
 // Measured on the first (one-thread-per-ray) version: incoherent bounce rays ran at 7-8 active
@@ -1014,6 +1057,43 @@ __global__ void __launch_bounds__(256) k_resolve(FrameLayout f, PathState ps, ui
             }
         }
     }
+}
+
+// k_resolve for every view of the table, one thread per (view, local pixel): view v folds its frames with b_v in place of
+// frame_id, into its local slots lp = v * npx_local + lp_v and its full frame at offset v * fb_w * fb_h.
+__global__ void __launch_bounds__(256) k_resolve_views(const __grid_constant__ ViewTable views, FrameLayout f, PathState ps,
+                                                      float *accum_local, uint32_t *img_local, float *accum_full,
+                                                      uint32_t *img_full)
+{
+    const uint32_t lp = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t npx_all = f.npx_local * views.num_views;
+    uint32_t x, y;
+    if (lp >= npx_all || !local_pixel_coords(f, lp % f.npx_local, x, y)) {
+        return;
+    }
+    const uint32_t v = lp / f.npx_local, first = views.view[v].frame_id;
+    float3 illum = mk3(accum_local[3 * (size_t)lp], accum_local[3 * (size_t)lp + 1], accum_local[3 * (size_t)lp + 2]);
+    for (uint32_t k = 0; k < f.frames; ++k) {
+        const float3 accum = illum;
+        illum = mk3(0.f);
+        for (uint32_t s = 0; s < f.spp; ++s) {
+            const float4 r = ps.radiance[(size_t)(k * f.spp + s) * npx_all + lp];
+            illum = illum + mk3(r.x, r.y, r.z);
+        }
+        illum = illum / (float)f.spp;
+        illum = (illum + (float)(first + k) * accum) / (float)(first + k + 1u);
+    }
+    accum_local[3 * (size_t)lp] = illum.x;
+    accum_local[3 * (size_t)lp + 1] = illum.y;
+    accum_local[3 * (size_t)lp + 2] = illum.z;
+    const uint32_t rgba = float_to_srgb8(illum.x) | (float_to_srgb8(illum.y) << 8) | (float_to_srgb8(illum.z) << 16) |
+                          0xff000000u;
+    img_local[lp] = rgba;
+    const size_t p = (size_t)v * f.fb_w * f.fb_h + (size_t)y * f.fb_w + x;
+    accum_full[3 * p] = illum.x;
+    accum_full[3 * p + 1] = illum.y;
+    accum_full[3 * p + 2] = illum.z;
+    img_full[p] = rgba;
 }
 
 // Scatter another rank's tile-local buffers into the full frame (frame-end gather, §8e)

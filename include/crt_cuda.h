@@ -138,6 +138,8 @@ void crtc_destroy(crtc_renderer *r);
  *                 more runs. Every builder ("bvh_builder" 0, 1, 2). Memory: the unique geometry (12 B per unique vertex,
  *                 + 8 B if it has uvs; 12 B per unique triangle; 128 B per instance; 32 B per (instance, geometry) pair),
  *                 36 B per flattened triangle and 32 B per BVH8 node.
+ *   "views"       V in 1..64, 1 (default): the number of cameras crtc_render_views traces together (see there). Takes
+ *                 effect at the next crtc_initialize; out of range is an error. V = 1 changes nothing.
  */
 int crtc_set_option(crtc_renderer *r, const char *key, int64_t value);
 
@@ -239,6 +241,44 @@ int crtc_render_async(crtc_renderer *r, const float *pos, const float *dir, cons
                       int camera_changed, uint32_t num_frames);
 int crtc_sync(crtc_renderer *r, crt_render_stats_t *total, float *stage_ms_sum, uint64_t *counters_sum,
               uint32_t *num_frames);
+
+/* One camera of crtc_render_views: the arguments crtc_render takes for it. */
+typedef struct crtc_view_t {
+    float pos[3], dir[3], up[3];
+    float fovy;
+    int camera_changed;
+} crtc_view_t;
+
+/* Multi-view rendering: several cameras' frames of the same scene as ONE wavefront. A renderer initialized with option
+ * "views" = V > 1 keeps V accumulation buffers and V full frames, view-major, and a frame counter b_k per view.
+ *   crtc_render_views enqueues num_frames (1..64) frames of each of the num_views views (num_views must equal V) as a
+ *   single wavefront on the renderer's stream and returns without waiting; crtc_sync collects it like a crtc_render_async
+ *   call: num_rays and the counters are summed over the views, the frame count grows by num_frames per call, the stage
+ *   times are those of the one wavefront, and counter [2] (launches) equals that of a one-view crtc_render_async call with
+ *   the same num_frames: no launch is added per view. Such calls never advance the "any_far_first" = 2 trial.
+ *   Resets. views[k].camera_changed resets view k only (b_k = 0), as crtc_render does; crtc_initialize, crtc_set_scene
+ *   and a crtc_commit_scene that applies something reset every view.
+ *   Guarantee. After any sequence of crtc_render_views calls, view k's accum and img equal, bit for bit, those of a
+ *   renderer with V = 1 and otherwise the same options, scene and size that received crtc_render_async calls with view k's
+ *   camera, camera_changed flag and num_frames, in the same order: path (view k, pixel, sample s of the batch) is seeded as
+ *   that renderer seeds it, from frame b_k; traversal, shading and next-event estimation are per path and do not depend
+ *   on its queue position; the resolve folds view k's samples with b_k.
+ *   Memory per view: 16 B per pixel of the 64x64-padded tiles (accum + img) + 16 B per framebuffer pixel (the full frame),
+ *   and the path state of V times as many paths (about 200 B per path in flight, as for crtc_render_async).
+ *   With V = 1, crtc_render_views is crtc_render_async with views[0] and crtc_read_view(r, 0, ...) reads the frame.
+ *   With V > 1 the following are errors (the renderer stays usable): crtc_initialize with option "aov", with
+ *   world_size > 1 or with adaptive sampling set; crtc_set_adaptive with params != NULL; crtc_render, crtc_render_async,
+ *   crtc_read_accum, crtc_read_img, crtc_copy_img_to_array, crtc_export_frame, crtc_import_frame, crtc_share_frame,
+ *   crtc_local_buffers and crtc_assemble_rank; and a call with V * num_frames * spp * (64x64-padded pixels) >= 2^31
+ *   paths. crtc_trace_closest, crtc_trace_any, crtc_bench_trace, the scene-update calls and the options "hw_textures",
+ *   "bvh_builder", "count_traversal" and "stage_events" work as with one view.
+ *   Not supported: views across GPUs, AOVs and the denoiser per view, adaptive sampling per view, a different size or
+ *   spp per view, non-pinhole cameras, and a channel in the drop-in plugin (which has one camera by construction). */
+int crtc_render_views(crtc_renderer *r, const crtc_view_t *views, uint32_t num_views, uint32_t num_frames);
+/* View `view` (< option views at the last crtc_initialize) of a multi-view renderer: its accum (fb_width*fb_height*3
+ * floats, as crtc_read_accum) and img (fb_width*fb_height RGBA8, as crtc_read_img), either may be NULL. Waits for the
+ * stream first, like crtc_read_accum. */
+int crtc_read_view(crtc_renderer *r, uint32_t view, float *rgb_out, uint32_t *img_out);
 
 /* The accumulated float framebuffer (what parity compares): fb_width*fb_height*3 floats,
  * row-major RGB. The reference keeps it backend-private and tile-major
